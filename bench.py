@@ -2,9 +2,9 @@
 """Headline benchmark: user-item pairs scored / second (fused top-k) at rank 50.
 
     python bench.py --gpus N --steps K --warmup W            (our arm)
-    python bench.py --impl reference --gpus N --steps K ...  (the reference's own CPU path, baseline/_ref)
+    python bench.py --impl reference --gpus N --steps K ...  (the reference's own CPU path, oracle/_ref)
 
-Workload (BASELINE.json configs[1], "C2"): synthetic 1M users x 100K items, ~0.1% nnz (1e8 interactions, Zipf item
+Workload "C2": synthetic 1M users x 100K items, ~0.1% nnz (1e8 interactions, Zipf item
 popularity, log-normal user degrees), SVDModel rank 50, filter_seen, top-10, every user scored against every item.
 One *step* = one full pass of the hot path on device-resident inputs: SpMM E = P.V, fused score + mask + top-k, merge.
 
@@ -55,7 +55,7 @@ def parse_args():
     ap.add_argument("--nnz", type=int, default=100_000_000)
     ap.add_argument("--rank", type=int, default=50)
     ap.add_argument("--topk", type=int, default=10)
-    ap.add_argument("--kernel", default=None, choices=[None, "simt", "tcgen05"])
+    ap.add_argument("--kernel", default=None, choices=[None, "simt", "tc"])
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
                     help="strong: --items is the TOTAL item count, split over the GPUs")
     ap.add_argument("--cpu-seconds", type=float, default=24.0, help="budget of the CPU-baseline sample")
@@ -67,7 +67,29 @@ def parse_args():
                     help="c2 (default; with --users/--items/--nnz/--rank/--gpus also C3's shape), c4 = CoFFee HOOI on a "
                          "1M x 50K x 5 tensor, c5 = ScaledSVD rank sweep on 5M x 500K (one build at rank 500)")
     ap.add_argument("--scale", type=float, default=1.0, help="c4/c5: shrink users, items and nnz by this factor")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="c2, one process: write the lists of the last timed step (a fixed, seeded sample of user rows) to DIR/*.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.config != "c2" or args.impl != "b200" or int(os.environ.get("WORLD_SIZE", "1")) > 1):
+        ap.error("--dump-outputs needs the default c2 configuration of this implementation in one process")
+    return args
+
+
+DUMP_ROWS = 200_000          # sampled user rows of --dump-outputs: 200K x top-10 float64 = 16 MB
+
+
+def dump_outputs(out_dir, ids, n_users):
+    """The timed path's result of its last step: ids [users x topk] (int64 item ids, stored exactly as float64) for a
+    fixed seeded sample of users, and the sampled row numbers."""
+    os.makedirs(out_dir, exist_ok=True)
+    rows = np.arange(n_users) if n_users <= DUMP_ROWS else \
+        np.sort(np.random.default_rng(0).choice(n_users, DUMP_ROWS, replace=False))
+    import torch
+    sample = ids.index_select(0, torch.from_numpy(rows).to(ids.device)).cpu().numpy()
+    np.save(os.path.join(out_dir, "topk_ids.npy"), sample.astype(np.float64))
+    np.save(os.path.join(out_dir, "user_rows.npy"), rows.astype(np.float64))
 
 
 # ------------------------------------------------------------------ data ------------
@@ -143,6 +165,12 @@ def summarize_clocks(samples):
     return {"sm_mhz": float(np.median(sm)), "sm_max_mhz": float(max(mx)), "reasons": sorted(reasons)}
 
 
+# NVIDIA H100 SXM data sheet (700 W card): dense BF16 tensor rate and HBM3 bandwidth; the roofline denominators unless
+# MEASURED_PEAKS.json holds numbers measured on the card at hand
+H100_BF16_TFLOPS = 989.0
+H100_HBM_GBS = 3350.0
+
+
 def load_peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
@@ -152,10 +180,10 @@ def load_peaks():
 
 # ------------------------------------------------------------- CPU baseline ---------
 def reference_baseline(triplets, shape, v64, topk, budget_s):
-    """The reference itself (polara, from baseline/_ref) on this box's host cores: SVDModel.get_recommendations()'s own
+    """The reference itself (polara, from oracle/_ref) on this box's host cores: SVDModel.get_recommendations()'s own
     chunk driver over the first chunks of users with the FULL test arrays in place (so each chunk pays what it pays in
     the full job, models.py:260-270), (i) library defaults (memory_hard_limit 1 GiB, no thread pool,
-    polara/recommender/defaults.py:50-51) and (ii) tuned (larger chunks + max_test_workers), as BASELINE.md 2 promises.
+    polara/recommender/defaults.py:50-51) and (ii) tuned (larger chunks + max_test_workers).
     Falls back to the oracle port when the reference cannot be imported (kind says which)."""
     n_users, n_items = shape
     try:
@@ -275,7 +303,7 @@ def run_c4(args):
     model.mlrank = (60, 60, 4)
     model.seed = 0
     model.growth_tol = 0.0                         # run exactly num_iters iterations
-    iters_w, iters_t = max(1, min(args.warmup, 2)), max(2, args.steps)
+    iters_w, iters_t = max(1, min(args.warmup, 2)), args.steps
     model.num_iters = iters_w
     model.build(); torch.cuda.synchronize()
     model.num_iters = iters_w + iters_t
@@ -291,7 +319,7 @@ def run_c4(args):
     u1 = eng.upload(model.factors["itemid"].astype(np.float32)); u2 = eng.upload(model.factors["rating"].astype(np.float32))
     ttm_ms = timed(lambda: eng.ttm(n_users, seg, a2, a1, vv, u2, r2, u1, r1), 5, torch.cuda.synchronize)
     ttm_bytes = nnz * 16.0 + 4.0 * (n_items * r1 + 5 * r2) + 4.0 * n_users * r1 * r2
-    peaks = load_peaks(); peak_hbm = float(peaks.get("hbm_gbs", 6500.0))
+    peaks = load_peaks(); peak_hbm = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     out = {"metric": "HOOI iterations per second (CoFFee build), core (60,60,4)", "value": 1.0 / s_per_iter, "unit": "iterations/s",
            "n_gpus": 1, "steps": iters_t, "warmup": iters_w, "ms_per_step": s_per_iter * 1e3, "higher_is_better": True,
            "scaling": "weak", "vs_baseline": None, "dtype": "f32 (f64 Gram / eigen)", "data": "synthetic",
@@ -307,7 +335,7 @@ def run_c4(args):
 def run_c5(args):
     """BASELINE config C5: ScaledSVD (col_scaling 0.4, EIGENREC) on 5M x 500K, nnz 5e8: ONE build at rank 500, then
     scoring at rank in {10, 50, 100, 200, 500} by rank truncation without rebuilding (models.py:819-832,
-    pipelines.py:81-116).  Every rank runs the tcgen05 kernel (K-slab pipeline above rank 61)."""
+    pipelines.py:81-116).  Every rank runs the tensor-core kernel (K-slab pipeline above rank 61)."""
     import torch
     import warnings
     from polara_b200 import _build
@@ -335,7 +363,7 @@ def run_c5(args):
         model.build()
     torch.cuda.synchronize(); build_s = time.perf_counter() - t0
     p_dev = DeviceCSR(indptr_d, indices_d, values_d, shape)
-    peaks = load_peaks(); peak_tf = float(peaks.get("bf16_tflops", 1590.0))
+    peaks = load_peaks(); peak_tf = float(peaks.get("bf16_tflops", H100_BF16_TFLOPS))
     pairs = float(n_users) * float(n_items)
     sweep = []
     for rank in (500, 200, 100, 50, 10):
@@ -344,7 +372,7 @@ def run_c5(args):
         step = pdist.make_step(eng, p_dev, v_dev, rank, args.topk, None)
         step(); torch.cuda.synchronize()
         s0 = eng.stats()
-        ms = timed(step, max(1, min(args.steps, 3)), torch.cuda.synchronize)
+        ms = timed(step, args.steps, torch.cuda.synchronize)
         s1 = eng.stats()
         eng.set_prune(False)
         ms_full = timed(step, 1, torch.cuda.synchronize)
@@ -387,7 +415,7 @@ def main():
             "config": {"workload": workload, "users": args.users, "items_total": n_items_total,
                        "items_per_gpu": n_items_total // n_gpus, "nnz": args.nnz, "rank": args.rank, "topk": args.topk,
                        "parallelism": "item-shard x%d" % n_gpus,
-                       "l2_policy": "inputs (P, E, lists > 1 GB) larger than the 126 MB L2"}}
+                       "l2_policy": "inputs (P, E, lists > 1 GB) larger than the 50 MB L2"}}
 
     if args.impl == "reference":
         if rank != 0:
@@ -487,6 +515,8 @@ def main():
     ms = ev0.elapsed_time(ev1)
     stats1 = eng.stats()
     launches = stats1[0] - stats0[0]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, ids, args.users)
     if world > 1:
         t = torch.tensor([ms], device=dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -505,9 +535,9 @@ def main():
 
     # ---------------- rooflines --------------------------------------------------------
     peaks = load_peaks()
-    peak_tf = float(peaks.get("bf16_tflops", 1590.0))
-    peak_hbm = float(peaks.get("hbm_gbs", 6500.0))
-    peak_src = "measured (MEASURED_PEAKS.json, burst)" if peaks else "fallback (B200_PROFILING.md)"
+    peak_tf = float(peaks.get("bf16_tflops", H100_BF16_TFLOPS))
+    peak_hbm = float(peaks.get("hbm_gbs", H100_HBM_GBS))
+    peak_src = "measured (MEASURED_PEAKS.json, burst)" if peaks else "H100 SXM data sheet (dense bf16, HBM3)"
     items_local = n_items_total // world
     # (a) SpMM E = P V alone (this rank's rows when sharded): algorithmic bytes of SURVEY.md 8d
     p_sp = pdist.row_block(eng, p_dev, sharder) if sharder is not None else p_dev
@@ -553,20 +583,10 @@ def main():
                           "unit": "TFLOP/s", "kernel_ms": fused_ms_default, "peak_source": peak_src, "traffic": None,
                           "note": "achieved counts only the EXECUTED tile products (algorithmic flops x executed share)"}
     roof_default_fused["frac"] = roof_default_fused["achieved"] / peak_tf
-    # DRAM traffic per launch (dram__bytes_read.sum + dram__bytes_write.sum) from the committed `ncu --set full` captures of
-    # exactly this command (profiles/spmm_step_r2_ncu.txt, score_topk_tc_r2_ncu.txt, score_topk_tc_pruned_r2_ncu.txt): only
-    # for the configuration they were taken on (C2 defaults, one GPU, tcgen05 kernel); null for anything else.
-    if (world == 1 and (args.users, args.items, args.nnz, args.rank, args.topk) == (1_000_000, 100_000, 100_000_000, 50, 10)
-            and (args.kernel or "tcgen05") == "tcgen05"):
-        src = "ncu --set full, C2, one B200 (profiles/*_r2_ncu.txt)"
-        roof_spmm.update(traffic=840.361472e6 + 241.191680e6, traffic_source=src)
-        if roof_fused is not None:
-            roof_fused.update(traffic=284.461824e6 + 137.639424e6, traffic_source=src)
-        roof_default_fused.update(traffic=282.235904e6 + 129.994752e6, traffic_source=src)
     roofline = roof_spmm if spmm_share >= fused_share else roof_default_fused
     roofline = dict(roofline, share_of_step=max(spmm_share, fused_share))
     out.update({"value": value, "ms_per_step": ms_per_step,
-                "dtype": "f32 (bf16 tensor-core filter, exact fp32 rescoring)" if (args.kernel or "tcgen05") == "tcgen05" else "f32",
+                "dtype": "f32 (bf16 tensor-core filter, exact fp32 rescoring)" if (args.kernel or "tc") == "tc" else "f32",
                 "gpu_launches": int(launches), "roofline": roofline,
                 "rooflines": {"spmm": roof_spmm, "fused_full_sweep": roof_fused, "fused_default": roof_default_fused},
                 "phase_ms": phase_ms, "sweep": {"tile_products_executed": int(swept), "tile_products_full": int(swept_full),
@@ -681,7 +701,7 @@ def main():
 
 
 def run_reference(args, base, n_items_total):
-    """Reference arm: the UNMODIFIED reference (polara, installed into baseline/_ref) scores a bounded sample of the
+    """Reference arm: the UNMODIFIED reference (polara, installed into oracle/_ref) scores a bounded sample of the
     workload per step through its own chunk driver on the host cores; no GPU, none of our code on the path (the data
     generator is numpy; the data stub replays test_to_coo)."""
     from oracle import ref_driver as rd
@@ -694,7 +714,8 @@ def run_reference(args, base, n_items_total):
     except Exception as exc:                                  # noqa: BLE001
         cb = port_baseline(trip, shape, v64, args.topk, 20.0, why=str(exc))
         out = dict(base)
-        out.update({"impl": "reference", "value": cb["value"], "ms_per_step": None, "dtype": "f64", "cpu_baseline": cb,
+        # the reference is not installed (oracle/install_ref.py): this is the oracle's port of its chunk driver
+        out.update({"impl": "oracle-port", "value": cb["value"], "ms_per_step": None, "dtype": "f64", "cpu_baseline": cb,
                     "e2e": {"value": cb["value"], "unit": "pairs/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
                     "gpu_launches": 0})
         print(json.dumps(out))
@@ -741,7 +762,7 @@ def run_reference(args, base, n_items_total):
     out = dict(base)
     out.update({"impl": "reference", "value": value, "ms_per_step": dt * 1e3, "dtype": "f64",
                 "cpu_baseline": {"value": value, "unit": "pairs/s", "cores": cores, "kind": "reference",
-                                 "sample": "polara SVDModel chunk driver (baseline/_ref, unmodified), %s knobs: %d users "
+                                 "sample": "polara SVDModel chunk driver (oracle/_ref, unmodified), %s knobs: %d users "
                                            "(%d chunks of %d) x %d items per step, full-size test arrays in place"
                                            % (which, per_step_users, cfg["chunks_per_step"], cfg["chunk_users"], n_items_total),
                                  "settings": settings, "host": host},

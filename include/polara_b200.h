@@ -1,5 +1,5 @@
 /*
- * polara_b200 -- C-ABI of the B200-native factorization-and-scoring engine.
+ * polara_b200 -- C-ABI of the H100-native factorization-and-scoring engine.
  *
  * The reference (evfro/polara, pure Python) has NO FFI of its own: its hot path
  * bottoms out in scipy/numpy/numba calls.  Each entry point below replaces one
@@ -16,7 +16,7 @@
  *   - CSR: indptr int64 [n_rows+1], indices int32 [nnz] (sorted within a row),
  *     values float32 [nnz].  Dense matrices are row-major float32 with an explicit
  *     leading dimension (ld, in elements).
- *   - sm_100a only.  No CPU fallback exists.
+ *   - sm_90a (H100) only.  No CPU fallback exists.
  */
 #ifndef POLARA_B200_H
 #define POLARA_B200_H
@@ -51,7 +51,7 @@ int pb200_ctx_sync(pb200_ctx* ctx);
 /* development aid: prints the diagnostics a timed-out (trapped) kernel left in pinned host memory to stderr */
 int pb200_debug_dump(pb200_ctx* ctx);
 /* which scoring kernel pb200_score_topk uses: 0 = exact SIMT fp32 kernel,
- * 1 = tcgen05 (bf16 tensor-core filter + exact fp32 rescoring; same results). */
+ * 1 = tc (bf16 wgmma tensor-core filter + exact fp32 rescoring; same results). */
 int pb200_set_score_kernel(pb200_ctx* ctx, int kind);
 /* 1 (default): a user tile's sweep over the norm-ordered items stops at the first position where
  * ||e_u|| * ||v_pos|| (Cauchy-Schwarz) can no longer reach the user's seeded k-th best score -- results are unchanged
@@ -112,7 +112,7 @@ typedef struct {
  *   4           the same with 32-bit gathers (a lane owns one column per 32-column group; also taken for operands that
  *               are not 16-byte aligned);
  *   1 / 2       dense rows of X staged in shared memory by cp.async.bulk (one UBLKCP per row) / by 16-byte cp.async --
- *               measured slower (the per-row copy issue is the bottleneck, DESIGN.md 3.2); operands that are not
+ *               the per-row copy issue limits them; operands that are not
  *               16-byte aligned fall back to 0;
  *   0           row-owned register gathers (round-1 kernel). */
 int pb200_set_spmm_kernel(pb200_ctx* ctx, int kind);
@@ -129,7 +129,7 @@ int pb200_spmm(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, int64_t nnz,
 int pb200_spmm_csr(pb200_ctx* ctx, const pb200_csr_view* a, const float* X, int64_t ldx, float* Y, int64_t ldy, int ell);
 
 /* Panel-major copy of a CSR matrix (see pb200_csr_view): a format conversion done once per build() so that the slice
- * of the dense operand one panel gathers from (panel_cols rows of X) stays resident in the 126 MB L2 while the nnz
+ * of the dense operand one panel gathers from (panel_cols rows of X) stays resident in the 50 MB L2 while the nnz
  * stream through.  b_indptr [n_panels * n_rows + 1], b_indices/b_values [nnz] device; panel_ptr_host [n_panels + 1] HOST.
  * n_panels must equal ceil(n_cols / panel_cols).  Synchronises the stream (the panel offsets are returned to the host). */
 int pb200_csr_block_columns(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, int64_t nnz,

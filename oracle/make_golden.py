@@ -1,12 +1,12 @@
 """Generate ``tests/golden/*.npz`` by running the REAL reference (imported from
-/root/reference) in the build container.  TEST INFRASTRUCTURE.
+the checkout named by POLARA_REFERENCE_ROOT).  TEST INFRASTRUCTURE.
 
     python oracle/make_golden.py
 
 Each fixture stores the hot path's *inputs* exactly as the reference's data
 model hands them to the model (``to_coo``, ``_get_test_data``), plus the
 reference's *outputs* (factors, recommendations, evaluate() hit counts), so the
-fixtures can be replayed on the GPU box where the reference does not exist.
+fixtures can be replayed where the reference does not exist.
 """
 import os
 import sys
@@ -174,6 +174,104 @@ def kernel_fixture(name="kernels_small", seed=5):
     print(name, "done")
 
 
+def live_fixture(name="reference_live"):
+    """Reference outputs that tests/test_oracle_vs_reference.py compares the oracle with: the reference's static kernels
+    on seeded inputs, HOOI, an SVDModel and a CoffeeModel through RecommenderData.prepare, round_core and the hit-rate /
+    reciprocal-rank functions.  The oracle's own inputs are stored with them, so the comparison runs without the reference."""
+    import scipy.sparse as sps
+    polara = import_reference()
+    from polara.recommender.models import RecommenderModel, SVDModel, CoffeeModel
+    from polara.recommender.data import RecommenderData
+    from polara.preprocessing.matrices import rescale_matrix
+    from polara.lib.tensor import hooi
+    from polara.recommender.evaluation import assemble_scoring_matrices, get_hr_score, get_rr_scores
+    out = {}
+    # downvote / topsort / rescale_matrix on random inputs
+    for seed in (1, 2):
+        rng = np.random.default_rng(seed)
+        s = rng.standard_normal((20, 50))
+        rows = np.repeat(np.arange(20), 4)
+        cols = np.concatenate([rng.choice(50, 4, replace=False) for _ in range(20)])
+        ref = s.copy()
+        RecommenderModel.downvote_seen_items(ref, (rows, cols))
+        out["dv%d_downvoted" % seed] = ref
+        out["dv%d_topsort6" % seed] = np.stack([RecommenderModel.topsort(ref[row], 6) for row in range(20)])
+        a = sps.random(40, 30, density=0.2, random_state=seed, format="csr")
+        for j, (scaling, axis) in enumerate(((0.4, 0), (0.8, 1), (1, 0))):
+            out["dv%d_rescaled%d" % (seed, j)] = rescale_matrix(a, scaling, axis).toarray()
+    # HOOI
+    rng = np.random.default_rng(3)
+    shp = (40, 30, 5)
+    idx = np.unique(np.stack([rng.integers(0, s, 900) for s in shp], axis=1), axis=0).astype(np.intp)
+    ref = hooi(idx, np.ones(len(idx)), shp, (4, 3, 2), num_iters=6, growth_tol=1e-4, seed=5)
+    for j in range(3):
+        out["hooi_f%d" % j] = ref[j]
+    out["hooi_core"] = ref[3]
+    # SVDModel through the reference's data model (ML-1M-like density, shrunk to keep the fixture small)
+    df = _frame(1200, 740, 166, rank=12, seed=11)
+    data = RecommenderData(df, "userid", "itemid", "rating", seed=0)
+    data.verbose = False
+    data.prepare()
+    model = SVDModel(data)
+    model.verbose = False
+    model.rank = 10
+    model.build()
+    out["svd_recs"] = model.get_recommendations().astype(np.int32)
+    idx, val, shp = data.to_coo(tensor_mode=False)
+    out["svd_train_idx"] = idx.astype(np.int32); out["svd_train_val"] = val.astype(np.float32)
+    out["svd_train_shape"] = np.array(shp)
+    out["svd_sigma"] = model.factors["singular_values"]
+    out["svd_v"] = model.factors[data.fields.itemid]
+    (tu, ti, tf), tshape, _ = model._get_test_data()
+    out["svd_test_u"] = np.asarray(tu, dtype=np.int32); out["svd_test_i"] = np.asarray(ti, dtype=np.int32)
+    out["svd_test_f"] = np.asarray(tf, dtype=np.float32); out["svd_test_shape"] = np.array(tshape)
+    # CoffeeModel with the reference's default multilinear rank
+    df = _frame(1500, 600, 40, rank=6, seed=13)
+    data = RecommenderData(df, "userid", "itemid", "rating", seed=0)
+    data.verbose = False
+    data.prepare()
+    model = CoffeeModel(data)
+    model.verbose = False
+    model.seed = 3
+    model.num_iters = 8
+    model.build()
+    out["cf_recs"] = model.get_recommendations().astype(np.int32)
+    idx, val, shp = data.to_coo(tensor_mode=True)
+    out["cf_train_idx"] = idx.astype(np.int32); out["cf_train_val"] = val.astype(np.float32)
+    out["cf_train_shape"] = np.array(shp)
+    out["cf_mlrank"] = np.array(model.mlrank); out["cf_num_iters"] = np.array(model.num_iters)
+    out["cf_growth_tol"] = np.array(model.growth_tol); out["cf_seed"] = np.array(model.seed)
+    f = data.fields
+    for j, key in enumerate((f.userid, f.itemid, f.feedback)):
+        out["cf_f%d" % j] = model.factors[key]
+    out["cf_core"] = model.factors["core"]
+    (tu, ti, tf), tshape, _ = model._get_test_data()
+    out["cf_test_u"] = np.asarray(tu, dtype=np.int32); out["cf_test_i"] = np.asarray(ti, dtype=np.int32)
+    out["cf_test_f"] = np.asarray(tf, dtype=np.int64); out["cf_test_shape"] = np.array(tshape)
+    # round_core
+    rng = np.random.default_rng(9)
+    core = rng.standard_normal((7, 6, 4))
+    out["rc_core"] = core
+    for j, (mode, rank) in enumerate(((0, 3), (1, 6), (1, 2), (2, 1), (2, 3))):
+        rot, new_core = CoffeeModel.round_core(core, mode, rank)
+        out["rc%d_rot" % j] = rot; out["rc%d_core" % j] = new_core
+    # hit rate, ARHR, MRR
+    for sp in (None, 4):
+        rng = np.random.default_rng(12)
+        m, n, k = 60, 90, 10
+        recs = np.stack([rng.choice(n, k, replace=False) for _ in range(m)])
+        hu = np.repeat(np.arange(m), 3)
+        hi = np.concatenate([rng.choice(n, 3, replace=False) for _ in range(m)])
+        hf = rng.integers(1, 6, size=len(hu)).astype(np.float64)
+        holdout = pd.DataFrame({"userid": hu, "itemid": hi, "rating": hf})
+        is_positive = None if sp is None else (hf >= sp)
+        d = assemble_scoring_matrices(recs, holdout, "userid", "itemid", is_positive, feedback="rating")
+        hr, rr = get_hr_score(d[1]), get_rr_scores(d[1])
+        out["rates_%s" % sp] = np.array([hr.hr, rr.arhr, rr.mrr], dtype=np.float64)
+    np.savez_compressed(os.path.join(GOLDEN, name + ".npz"), **out)
+    print(name, "done")
+
+
 if __name__ == "__main__":
     os.makedirs(GOLDEN, exist_ok=True)
     kernel_fixture()
@@ -186,3 +284,4 @@ if __name__ == "__main__":
     # models.py:191-211) is covered through the oracle in tests/test_oracle_golden.py.
     coffee_fixture("coffee_small")
     coffee_fixture("coffee_flat34", flattener=[2, 3], seed=12)
+    live_fixture()

@@ -15,8 +15,8 @@ oracle calls the same routine at the same call sites (models.py:844,
 lib/tensor.py:71,75,79) because that *is* the reference's algorithm.
 
 Pinning: the reference's own tests hold no vector for this path (SURVEY.md §4).
-The oracle is therefore pinned against outputs of the reference itself, run in
-the build container by ``oracle/make_golden.py`` and committed under
+The oracle is therefore pinned against outputs of the reference itself, recorded
+by ``oracle/make_golden.py`` and committed under
 ``tests/golden/`` (see tests/test_oracle_golden.py, tests/test_oracle_vs_reference.py).
 """
 from __future__ import annotations

@@ -1,14 +1,14 @@
 """Drive the UNMODIFIED reference (evfro/polara) on plain arrays  --  TEST INFRASTRUCTURE.
 
 Used by ``bench.py --impl reference`` / the ``cpu_baseline`` leg (timing the reference's
-own CPU path on the GPU box's host cores) and by the drop-in tests.  The reference is
-imported from ``baseline/_ref`` (the offline ``pip install --target`` of ``/root/reference``,
-git-ignored, travels to the GPU box) or, in the build container, from ``/root/reference``.
+own CPU path on the host cores) and by the drop-in tests.  The reference is imported from
+``oracle/_ref`` (an offline ``pip install --target`` of a reference checkout, git-ignored) or from the checkout
+named by ``POLARA_REFERENCE_ROOT``; the callers skip or fall back when neither exists.
 Nothing of ``polara_b200`` (models, kernels, engine) is on this path.
 
 The reference's models read their inputs from a ``RecommenderData`` object
 (polara/recommender/data.py); its splitting / re-indexing logic is out of scope
-(SURVEY.md §2), so :class:`StubData` replays what that object hands to a model:
+so :class:`StubData` replays what that object hands to a model:
 ``to_coo`` (data.py:794-817), ``test_to_coo`` (data.py:835-862), ``get_test_shape``
 (data.py:865-884), ``fields``, ``warm_start`` and the event hooks (data.py:35-76).
 """
@@ -22,8 +22,8 @@ from collections import namedtuple
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_REF_CANDIDATES = (os.path.join(os.path.dirname(_HERE), "baseline", "_ref"),
-                   os.environ.get("POLARA_REFERENCE_ROOT", "/root/reference"))
+_REF_CANDIDATES = (os.path.join(_HERE, "_ref"),
+                   os.environ.get("POLARA_REFERENCE_ROOT", ""))
 
 Fields = namedtuple("Fields", "userid itemid feedback")
 _Index = namedtuple("Index", "userid itemid feedback")
@@ -147,7 +147,7 @@ def time_reference_scoring(model, max_chunks=None, max_seconds=None):
 
 
 def host_description():
-    """what BASELINE.md §2 asks to print with every CPU result."""
+    """the host facts printed with every CPU result (cores, CPU model, thread settings)."""
     info = {"cores": os.cpu_count()}
     try:
         with open("/proc/cpuinfo") as f:

@@ -1,8 +1,7 @@
-"""Import the real reference (``/root/reference``) in the BUILD CONTAINER only.
+"""Import the real reference (a checkout named by ``POLARA_REFERENCE_ROOT``) where one is available.
 
 TEST INFRASTRUCTURE.  Used by ``oracle/make_golden.py`` (fixture generation) and
-by ``tests/test_oracle_vs_reference.py`` (skipped when the checkout is absent,
-e.g. on the GPU box).  The reference is untouched; pandas>=3 removed two private
+by ``bench.py``'s reference arm.  The reference is untouched; pandas>=3 removed two private
 attributes it reads (``GroupBy.grouper`` at recommender/data.py:487,704-708 and
 ``BaseGrouper.group_info``), which we re-expose here before importing it.
 """
@@ -11,7 +10,7 @@ import sys
 
 import numpy as np
 
-REFERENCE_ROOT = os.environ.get("POLARA_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("POLARA_REFERENCE_ROOT", "")
 
 
 def reference_available():

@@ -1,4 +1,4 @@
-"""polara_b200 -- B200-native (sm_100a) engine behind the Polara SVD/CoFFee model API.
+"""polara_b200 -- H100-native (sm_90a) engine behind the Polara SVD/CoFFee model API.
 
 Host code is Python; all computation happens in hand-written CUDA reached through the
 C-ABI of ``libpolara_b200.so`` (see include/polara_b200.h).  No CPU fallback.

@@ -1,6 +1,6 @@
 """ctypes binding of ``libpolara_b200.so`` (the C-ABI declared in include/polara_b200.h).
 
-There is no CPU fallback: if the library is missing or no sm_100 device is
+There is no CPU fallback: if the library is missing or no sm_90 device is
 present, every product entry point raises.
 """
 from __future__ import annotations

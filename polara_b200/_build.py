@@ -1,4 +1,4 @@
-"""Builds ``libpolara_b200.so`` in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds ``libpolara_b200.so`` in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 import glob
 import os
 import shutil
@@ -8,8 +8,9 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libpolara_b200.so")
 
+ARCH = "arch=compute_90a,code=sm_90a"
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", ARCH, "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "--expt-relaxed-constexpr",
 ]
 
@@ -59,7 +60,7 @@ def build(force=False, verbose=False, extra_flags=()):
             raise RuntimeError("nvcc failed on %s:\n%s" % (src, out))
         if verbose and out.strip():
             print(out)
-    cmd = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-Xcompiler", "-fPIC",
+    cmd = [_nvcc(), "-gencode", ARCH, "-shared", "-Xcompiler", "-fPIC",
            "-o", LIB_PATH] + objs
     res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if res.returncode != 0:

@@ -49,14 +49,14 @@ extern "C" int pb200_ctx_create(int device, void* stream, pb200_ctx** out) {
     // profiling aid: PB200_PRUNE=0 starts the context with the early termination of the scoring sweep off (same as
     // pb200_set_prune(ctx, 0)); results are identical either way
     if (const char* e = getenv("PB200_PRUNE")) ctx->prune = atoi(e) != 0;
-    if (prop.major != 10) {
-        // built for sm_100a only: refuse loudly rather than fail at the first launch
+    if (prop.major != 9 || prop.minor != 0) {
+        // built for sm_90a only: refuse loudly rather than fail at the first launch
         delete ctx;
         return PB200_ENOTIMPL;
     }
     {
         // scratch buffers come from the stream-ordered pool; keep freed blocks cached across synchronisations
-        // (the default threshold 0 hands them back to the driver at every sync, which costs ~100 ms per GB re-allocated)
+        // (the default threshold 0 hands them back to the driver at every sync, and re-allocating them is slow)
         cudaMemPool_t pool;
         if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
             uint64_t keep = UINT64_MAX;
@@ -108,7 +108,7 @@ extern "C" int pb200_ctx_set_stream(pb200_ctx* ctx, void* stream) {
 
 extern "C" int pb200_set_score_kernel(pb200_ctx* ctx, int kind) {
     if (!ctx) return PB200_EINVAL;
-    PB_REQUIRE(ctx, kind == 0 || kind == 1, "score kernel must be 0 (simt) or 1 (tcgen05)");
+    PB_REQUIRE(ctx, kind == 0 || kind == 1, "score kernel must be 0 (simt) or 1 (tc: wgmma filter + exact rescoring)");
     ctx->score_kernel = kind;
     return PB200_OK;
 }

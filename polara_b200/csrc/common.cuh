@@ -1,4 +1,4 @@
-// Shared plumbing for the polara_b200 CUDA library (sm_100a only).
+// Shared plumbing for the polara_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -12,8 +12,8 @@
 struct pb200_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
-    int num_sms = 148;
-    int score_kernel = 1;          // 0 = SIMT exact, 1 = tcgen05 filter + exact rescoring
+    int num_sms = 132;
+    int score_kernel = 1;          // 0 = SIMT exact, 1 = tensor-core (wgmma) filter + exact rescoring
     int spmm_kernel = 3;           // 3 = nnz windows + register gathers (default), 1 / 2 = X rows staged in shared memory by
                                    // cp.async.bulk / cp.async, 0 = row-owned register gathers (round-1 kernel)
     int prune = 1;                 // 1 = stop a user tile's sweep where ||e|| * ||v|| can no longer reach its threshold

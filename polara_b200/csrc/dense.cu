@@ -229,8 +229,8 @@ jacobi_psd_kernel(double* __restrict__ X, double* __restrict__ R, int c, double*
 }
 
 // ---- the same one-sided Jacobi spread over the whole GPU: one launch per ROUND of a sweep (the c/2 row pairs of a round
-// are disjoint), one block per pair.  The single-CTA kernel above takes 59 ms for c = 240 and > 1 s for c = 768 (a HOOI
-// unfolding / the rank-500 build of C5); a round here is a few microseconds.  Same pair order => same rotations.
+// are disjoint), one block per pair.  The single-CTA kernel above does all c (c - 1) / 2 rotations of a sweep in one SM,
+// which does not scale to c in the hundreds (a HOOI unfolding / the rank-500 build of C5).  Same pair order => same rotations.
 __global__ void jacobi_init_kernel(double* __restrict__ R, int c, int* __restrict__ flags) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e < c * c) R[e] = (e / c == e % c) ? 1.0 : 0.0;

@@ -767,8 +767,8 @@ int pb_spmm_panel(pb200_ctx* ctx, int64_t n_rows, const int64_t* indptr, const i
     int done = 0;
     while (done < ell) {
         const int w = ell - done;                         // live columns left
-        // measured at C2 (profiles/microbench_r2.txt): 128-bit gathers win for <= 64 columns (half a warp per nnz: 1.78 vs
-        // 2.30 ms) and lose for 96 (24 of 32 lanes busy: 3.17 vs 2.58 ms); 97..128 columns fill the warp again
+        // lane occupancy: with 128-bit gathers a group of <= 64 columns keeps half a warp per nnz busy, 65..96 columns
+        // only 24 of 32 lanes (those take the 32-bit kernel), 97..128 columns fill the warp again
         if (vec4 && w <= 64) {
             PB_TRY((launch_window4<false>(ctx, n_rows, indptr, indices, values, X + done, ldx, Y + done, ldy, nnz_begin, nnz_end,
                                           w, accumulate, sc)));

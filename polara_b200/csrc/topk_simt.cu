@@ -4,7 +4,7 @@
 // Replaces, fused: the dgemm of SVDModel.slice_recommendations (polara/recommender/
 // models.py:857-861), downvote_seen_items (models.py:494-519) and get_topk_elements
 // (models.py:522-564).  This is the reference implementation of the device contract; the
-// tcgen05 kernel (topk_tc.cu) must produce bit-identical lists.  `id_map` (optional) renames the
+// tensor-core kernel (topk_tc.cu) must produce bit-identical lists.  `id_map` (optional) renames the
 // rows of V (used when V is a gathered subset): ids in the lists and seen lookups use id_map[row].
 #include "topk_common.cuh"
 

@@ -1,4 +1,4 @@
-// Fused scoring on the 5th-gen tensor cores (tcgen05 / TMEM), sm_100a.
+// Fused scoring on the Hopper tensor cores (wgmma), sm_90a.
 //
 //   scores = E V^T  ->  seen-item mask  ->  per-user top-k          (score rows never reach HBM)
 //
@@ -7,30 +7,26 @@
 //
 // Idea: the tensor cores only FILTER.  Operands are packed to bf16 (A = -E, B = V) together with
 // three extra K-slots: a per-user threshold t_w (split hi+lo bf16, B holds 1.0 there) and a per-PAIR
-// error margin (A: -(2^-7 + 2^-13) ||e_u||, B: ||v_j||, both rounded up), so the fp32 accumulator in TMEM is
+// error margin (A: -(2^-7 + 2^-13) ||e_u||, B: ||v_j||, both rounded up), so the fp32 accumulator is
 //     d = t_w - s~ - (2^-7 + 2^-13) ||e_u|| ||v_j||   with  s~ = bf16 dot product, |s~ - s| <= (2^-7 + 2^-16) ||e|| ||v||
 // (bf16 unit round-off 2^-8 per operand; the 2^-13 and a 2^-16 |t_w| cut of the threshold pay for the fp32 accumulation).
 // Items are swept in order of decreasing ||v_j|| (stable radix sort of the norms, CUB), which makes
-// the running thresholds tight after the first tile.  The epilogue reads
-// TMEM with tcgen05.ld and keeps ONLY THE SIGN BIT of each accumulator (one SHF per pair):
-// sign set  <=>  s~ + margin > t_w  <=>  "candidate".  t_w is a lower bound of the user's final k-th
-// best exact score, so no true top-k item can be missed.
+// the running thresholds tight after the first tile.  The epilogue keeps ONLY THE SIGN BIT of each
+// accumulator register: sign set  <=>  s~ + margin > t_w  <=>  "candidate".  t_w is a lower bound of the
+// user's final k-th best exact score, so no true top-k item can be missed.
 // Candidates (a few hundred per user out of 1e5 items) are then checked against the user's seen
 // list and RESCORED EXACTLY in fp32 (the canonical fmaf chain of topk_common.cuh), which makes the
 // result bit-identical to the exact SIMT kernel (topk_simt.cu).  As better candidates arrive the
 // owner thread rewrites t_w inside the A operand in shared memory (generic-proxy store +
 // fence.proxy.async), so later MMAs filter harder.
 //
-// Pipeline per CTA (persistent, one CTA per SM, 10 warps):
-//   warp 8  producer : cp.async.bulk (UBLKCP) of pre-packed operand tiles, mbarrier complete_tx
-//   warps 9,10 MMA   : alternate tiles; one elected thread issues tcgen05.mma (M=128, N=128, K=16 per instr),
-//                      (the issue blocks while the pipe is busy -- ~384 cycles per tile, shared-memory bound in
-//                      SS mode -- so two issuers are needed to hide the ~350 cycles of barrier probing per tile)
-//                      tcgen05.commit releases smem stages / publishes TMEM accumulators
-//   warps 0-7 epilogue: tcgen05.ld 32x32b.x32, sign-bit masks, staging, flush (rescoring + lists)
-// TMEM holds a ring of four 128x128 fp32 accumulators (512 columns): an accumulator is busy for
-// (MMA latency + TMEM read-out latency) ~ 1000+ cycles while its MMAs take 256, so four small tiles in
-// flight hide what two 128x256 tiles could not (measured: 800 -> see DESIGN.md).
+// Pipeline per CTA (persistent, one CTA per SM, 9 warps):
+//   warp 8      producer : cp.async.bulk of pre-packed operand tiles (the A tile of the work item, then one 64-wide K
+//                          slab of an item tile per ring stage), mbarrier complete_tx
+//   warps 0-7   consumers: two warpgroups, each owns 64 users of the 128-user tile.  Per item tile a warpgroup issues
+//                          wgmma.mma_async m64n128k16 (A and B from shared memory, 128-byte swizzle), collects the K slabs
+//                          in 64 fp32 registers per thread, releases each ring stage as soon as its MMAs retired, then
+//                          turns the signs into per-user candidate masks, stages them and rescores.
 #include <cuda_bf16.h>
 #include <cstdlib>
 #include <cub/device/device_radix_sort.cuh>
@@ -39,38 +35,23 @@
 
 namespace {
 
-constexpr int BM = 128;          // users per tile (TMEM lanes)
-constexpr int BN = 128;          // items per tile (TMEM columns per accumulator)
-constexpr int NACC = 512 / BN;   // accumulator ring: the whole TMEM (4 x 128 columns)
-                                 // the two epilogue threads of a row take alternate tiles (all 128 columns)
-constexpr int NEPI_WARPS = 8;
-constexpr int NTHREADS = 352;    // 8 epilogue warps + producer + two MMA-issuing warps
-constexpr int CAPS = 16;         // staged (chunk, mask) entries per epilogue thread
+constexpr int BM = 128;          // users per tile (two warpgroups x 64)
+constexpr int BN = 128;          // items per tile (wgmma N)
+constexpr int NCONS = 256;       // consumer threads: two warpgroups
+constexpr int NTHREADS = NCONS + 32;   // + the producer warp
+constexpr int CAPS = 16;         // staged (chunk, mask) entries per consumer thread
 constexpr int MAX_STAGES = 10;
+constexpr uint32_t STAGE_BYTES = BN * 128;   // one ring stage: a 64-wide K slab (one 128-byte swizzle atom) of an item tile
 constexpr int PROBE_ITEMS = 256; // largest-norm items scored exactly up front to seed the thresholds
 constexpr int HEAD_TILES = 8;    // seen items among the first HEAD_TILES*BN sweep positions are masked by bitmap
 constexpr int HEAD_WORDS = HEAD_TILES * BN / 32;
-constexpr int TRACE_N = 4096;   // trace rows: [issue, tfull seen, release, loop top, operands ready, accumulators ready]
 constexpr long long SPIN_LIMIT_CYCLES = 4000000000ll;
-// Development switches (PB200_TC_DEBUG skips TMEM reads / MMAs, PB200_TC_TRACE dumps per-tile timestamps) change results
-// or cost time: they exist only in builds with -DPB200_DEVEL.  In the shipped library PB_DBG() is the constant 0 and the
-// trace pointer is never set, so the compiler drops those paths.
-#ifdef PB200_DEVEL
-#define PB_DBG(p) ((p).dbg)
-#define PB_TRACE(p) ((p).trace)
-#define PB_PROF(p) ((p).prof)
-#else
-#define PB_DBG(p) 0
-#define PB_TRACE(p) ((long long*)nullptr)
-#define PB_PROF(p) ((long long*)nullptr)
-#endif
 
 struct TcParams {
     const __nv_bfloat16* Ap;     // packed A tiles [user_tiles][BM x KP]
     const __nv_bfloat16* Bp;     // packed B tiles [item_tiles][BN x KP]
     const float* E; int64_t lde;
     const float* V; int64_t ldv;
-    const float* enorm;          // [m] ||e_u||
     const int32_t* perm;         // [n] sweep position -> item id (norm-descending order)
     const float* t0;             // [m] seed lower bound of the k-th best score (or -inf)
     int64_t m, n;
@@ -81,31 +62,18 @@ struct TcParams {
     const int64_t* seen_indptr; const int32_t* seen_indices; int64_t seen_offset;
     pb200_cand* lists;           // [parts*2][m][k]
     int stages;
-    int tok;                     // K-slab pipeline with a ring shorter than a tile + 1 (stages <= slabs): one issuing warp only
-    int slabs;                   // > 1: a pipeline stage holds ONE 64-wide K slab (128-byte atom) of an item tile instead of
-                                 //      the whole tile -- keeps ranks up to ~500 on the tensor cores (A stays resident)
     uint32_t a_bytes, b_bytes;
-    int ts;                      // 1: A operand lives in TMEM (tcgen05.mma TS form), 0: A in shared memory (SS)
-    int nacc;                    // accumulators in the TMEM ring (4 in SS mode, 3 in TS mode)
-    int a_bufs;                  // TS: TMEM copies of the A tile (2 = the next work's tile is prefetched)
-    int cluster;                 // CTAs per cluster sharing every B tile by multicast (1, 2 or 4)
-    int pair;                    // 1: CTA pairs issue tcgen05.mma.cta_group::2 (M = 256: each CTA its own 128 users,
-                                 //    each CTA stages HALF of every item tile); needs cluster == 2, K <= 64, SS mode
-    int dbg;                     // development switch (env PB200_TC_DEBUG): 1 = epilogue skips TMEM reads, 2 = no MMA issue
-    const int32_t* cut;          // [user tile groups] first item tile NOT needed by any user of the group (or null = sweep all)
-    const int32_t* order;        // [user tile groups] groups by decreasing cut (longest sweeps first), or null = natural order
+    const int32_t* cut;          // [user tiles] first item tile NOT needed by any user of the tile (or null = sweep all)
+    const int32_t* order;        // [user tiles] tiles by decreasing cut (longest sweeps first), or null = natural order
     const uint32_t* headbits;    // [m][HEAD_WORDS] seen bitmap of the head of the sweep order (or null)
     unsigned long long* stats;   // device counters
     unsigned long long* hdbg;    // pinned host memory for timeout diagnostics (or null)
-    long long* prof;             // development: per-CTA cycle accounting of epilogue thread 0 (8 values per CTA) or null
-    long long* trace;            // development: per-tile timestamps of CTA 0 (3 x TRACE_N) or null
 };
 
-// The i-th work item of a cluster.  Work = (group of `cluster` user tiles, item part).  With early termination the groups
-// cost between 1 and all item tiles: they are handed out longest first, each round of n_clusters items in the opposite
-// direction of the one before (cluster c gets ranks c, 2 nc - 1 - c, 2 nc + c, ...), which evens out the sums per cluster --
-// with the natural order the SMs were busy 37 % of the kernel's time at C2 (profiles/score_topk_tc_pruned_r2_ncu.txt).
-// All four roles of a CTA (producer, MMA issuers, both epilogue halves) walk the same sequence through this function.
+// The i-th work item of CTA c.  Work = (user tile, item part).  With early termination the user tiles cost between 1 and
+// all item tiles: they are handed out longest first, each round of nc items in the opposite direction of the one before
+// (CTA c gets ranks c, 2 nc - 1 - c, 2 nc + c, ...), which evens out the sums per CTA.
+// Both roles of a CTA (producer, consumers) walk the same sequence through this function.
 struct WorkItem { int64_t g; int part; };
 __device__ __forceinline__ bool next_work(const TcParams& p, int64_t i, int64_t c, int64_t nc, int64_t n_groups, WorkItem& wk) {
     const bool rev = p.order != nullptr && (i & 1) && (i + 1) * nc <= n_groups;
@@ -154,187 +122,54 @@ __device__ __noinline__ void mbar_wait_slow(uint32_t bar, uint32_t parity, unsig
     }
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, unsigned long long* stats, unsigned long long* hdbg) {
-    if (mbar_try_wait(bar, parity)) return;   // fast path: keeps the per-tile loops of the MMA / epilogue warps short
+    if (mbar_try_wait(bar, parity)) return;   // fast path
     mbar_wait_slow(bar, parity, stats, hdbg);
 }
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
-__device__ __forceinline__ void bulk_g2s_mc(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint16_t mask) {
-    // the bytes land at the same CTA-relative offset in every CTA of `mask`, and each of their mbarriers
-    // (same offset) receives the complete_tx
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
+
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving reads or writes of the accumulator registers across a wgmma fence / wait
+__device__ __forceinline__ void wg_fence_acc(float (&d)[64]) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// D[64 x 128] (+)= A[64 x 16] B[128 x 16]^T, both operands K-major bf16 in shared memory, fp32 accumulators in registers.
+// Thread t of the warpgroup holds d[4 i + 2 a + b] = D[16 (t / 32) + (t % 32) / 4 + 8 a][8 i + 2 (t % 4) + b].
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc, int accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t dst_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cta(uint32_t bar, uint32_t cta) {
-    asm volatile("{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-                 "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar), "r"(cta) : "memory");
-}
-// same, without a cluster-scope release: for hand-offs that carry no generic-proxy data (an accumulator that has been
-// read: tcgen05.wait::ld + tcgen05.fence::before_thread_sync order the TMEM side).  The releasing form costs the
-// epilogue ~900 cycles per tile (measured: read-out 1650 vs 720 cycles).
-__device__ __forceinline__ void mbar_arrive_cta_relaxed(uint32_t bar, uint32_t cta) {
-    asm volatile("{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-                 "mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar), "r"(cta) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16_pair_elect(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %4, 0;\n\telect.sync _|q, 0xffffffff;\n\t"
-                 "@q tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// Warp-uniform issue: the whole warp executes the surrounding code (so descriptors stay in uniform
-// registers) and ONE elected lane issues the tcgen05 instruction.  Issuing from a divergent single-lane
-// branch instead costs ~340 cycles per MMA (R2UR + waterfall loop) -- measured, see DESIGN.md.
-__device__ __forceinline__ void tc_mma_bf16_elect(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %4, 0;\n\telect.sync _|q, 0xffffffff;\n\t"
-                 "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_commit_elect(uint32_t bar) {
-    asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t"
-                 "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_commit_mc_elect(uint32_t bar, uint16_t mask) {
-    asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t"
-                 "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}"
-                 ::"r"(bar), "h"(mask) : "memory");
-}
-// One tile with K <= 64: four K=16 MMAs (the first overwrites the accumulator) and both commits, issued by
-// one elected lane from a single asm block (keeps the issue loop ~20 instructions per tile).
-__device__ __forceinline__ void tc_tile4_elect(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t bar_stage, uint32_t bar_acc, uint32_t mc, uint16_t mask) {
-    asm volatile("{\n\t.reg .pred q, pf, pt, pm;\n\t.reg .b64 a, b;\n\t"
-                 "elect.sync _|q, 0xffffffff;\n\t"
-                 "setp.ne.b32 pf, 0, 0;\n\tsetp.eq.b32 pt, 0, 0;\n\tsetp.ne.b32 pm, %6, 0;\n\t"
-                 "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, pf;\n\t"
-                 "add.u64 a, %1, 2;\n\tadd.u64 b, %2, 2;\n\t"
-                 "@q tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %3, pt;\n\t"
-                 "add.u64 a, %1, 4;\n\tadd.u64 b, %2, 4;\n\t"
-                 "@q tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %3, pt;\n\t"
-                 "add.u64 a, %1, 6;\n\tadd.u64 b, %2, 6;\n\t"
-                 "@q tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %3, pt;\n\t"
-                 "and.pred pt, q, pm;\n\tnot.pred pm, pm;\n\tand.pred pf, q, pm;\n\t"
-                 "@pf tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%4];\n\t"
-                 "@pt tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%4], %7;\n\t"
-                 "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%5];\n\t}"
-                 ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(bar_stage), "r"(bar_acc), "r"(mc), "h"(mask) : "memory");
-}
-// CTA-pair form of the same tile: M = 256 over the two CTAs of the cluster (each supplies its own A tile and half of
-// the B tile from its own shared memory), issued by the leader CTA only; both commits reach BOTH CTAs' barriers.
-__device__ __forceinline__ void tc_tile4_pair_elect(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                    uint32_t bar_stage, uint32_t bar_acc) {
-    asm volatile("{\n\t.reg .pred q, pf, pt;\n\t.reg .b64 a, b;\n\t"
-                 "elect.sync _|q, 0xffffffff;\n\t"
-                 "setp.ne.b32 pf, 0, 0;\n\tsetp.eq.b32 pt, 0, 0;\n\t"
-                 "@q tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, pf;\n\t"
-                 "add.u64 a, %1, 2;\n\tadd.u64 b, %2, 2;\n\t"
-                 "@q tcgen05.mma.cta_group::2.kind::f16 [%0], a, b, %3, pt;\n\t"
-                 "add.u64 a, %1, 4;\n\tadd.u64 b, %2, 4;\n\t"
-                 "@q tcgen05.mma.cta_group::2.kind::f16 [%0], a, b, %3, pt;\n\t"
-                 "add.u64 a, %1, 6;\n\tadd.u64 b, %2, 6;\n\t"
-                 "@q tcgen05.mma.cta_group::2.kind::f16 [%0], a, b, %3, pt;\n\t"
-                 "@q tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%4], %6;\n\t"
-                 "@q tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%5], %6;\n\t}"
-                 ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(bar_stage), "r"(bar_acc), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair_elect(uint32_t bar) {
-    asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t"
-                 "@q tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}"
-                 ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-// TS form: A comes from TMEM (rows on lanes, two bf16 per 32-bit column), B from shared memory
-__device__ __forceinline__ void tc_mma_bf16_ts_elect(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %4, 0;\n\telect.sync _|q, 0xffffffff;\n\t"
-                 "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-                 ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_tile4_ts_elect(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc,
-                                                  uint32_t bar_stage, uint32_t bar_acc, uint32_t mc, uint16_t mask) {
-    asm volatile("{\n\t.reg .pred q, pf, pt, pm;\n\t.reg .b64 b;\n\t.reg .b32 a;\n\t"
-                 "elect.sync _|q, 0xffffffff;\n\t"
-                 "setp.ne.b32 pf, 0, 0;\n\tsetp.eq.b32 pt, 0, 0;\n\tsetp.ne.b32 pm, %6, 0;\n\t"
-                 "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, pf;\n\t"
-                 "add.u32 a, %1, 8;\n\tadd.u64 b, %2, 2;\n\t"
-                 "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %3, pt;\n\t"
-                 "add.u32 a, %1, 16;\n\tadd.u64 b, %2, 4;\n\t"
-                 "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %3, pt;\n\t"
-                 "add.u32 a, %1, 24;\n\tadd.u64 b, %2, 6;\n\t"
-                 "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %3, pt;\n\t"
-                 "and.pred pt, q, pm;\n\tnot.pred pm, pm;\n\tand.pred pf, q, pm;\n\t"
-                 "@pf tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%4];\n\t"
-                 "@pt tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%4], %7;\n\t"
-                 "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%5];\n\t}"
-                 ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(bar_stage), "r"(bar_acc), "r"(mc), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]) : "memory");
-}
-__device__ __forceinline__ void tmem_st1(uint32_t taddr, uint32_t v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(v) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                   "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                   "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                   "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                 : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // Operand tiles are K-major with the 128-byte swizzle: a tile of ROWS x KP bf16 is stored as
 // ceil(KP/64) "atoms" of ROWS x 128 B; inside an atom row r sits at r*128 B and its eight 16-byte
-// chunks are XOR-ed with (r % 8)  (Swizzle<3,4,3>); 8-row groups are 1024 B apart (SBO).  With the
-// unswizzled "interleave" layout the tensor core fetched operands at a quarter of the rate (measured:
-// 512 instead of 128 cycles per M128 N256 K16 instruction), hence the swizzle.
+// chunks are XOR-ed with (r % 8)  (Swizzle<3,4,3>); 8-row groups are 1024 B apart (SBO).  This is the
+// layout wgmma reads with the SWIZZLE_128B descriptor; a K step of 16 inside an atom advances the start by 32 B.
 __host__ __device__ __forceinline__ size_t tile_byte(int rows, int row, int k) {
     return (size_t)(k / 64) * ((size_t)rows * 128) + (size_t)(row / 8) * 1024 + (size_t)(row % 8) * 128 +
            (size_t)((((k % 64) / 8) ^ (row % 8)) * 16) + (size_t)(k % 8) * 2;
 }
-// UMMA shared-memory descriptor: K-major, SWIZZLE_128B (layout type 2), SBO = 1024 B, version 1
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-           (2ull << 61);
-}
-// instruction descriptor: D=f32 (bits 4-5 = 1), A=B=bf16 (bits 7-9, 10-12 = 1), K-major both, N>>3 @17, M>>4 @24
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// wgmma shared-memory matrix descriptor: start address >> 4, LBO 16 B (unused with this swizzle), SBO = 1024 B,
+// layout type 1 = SWIZZLE_128B (bits 62-63); atoms are 1024-byte aligned, so the base offset is 0
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 
 // bf16 bit helpers (round toward -inf so that thresholds stay conservative)
@@ -393,7 +228,7 @@ __global__ void pack_items_kernel(const float* __restrict__ V, int64_t ldv, int6
 
 __global__ void pack_users_kernel(const float* __restrict__ E, int64_t lde, int64_t m, int r, int rs, int KP,
                                   int64_t user_tiles, const float* __restrict__ enorm,
-                                  const float* __restrict__ t0, __nv_bfloat16* __restrict__ Ap, int row_major) {
+                                  const float* __restrict__ t0, __nv_bfloat16* __restrict__ Ap) {
     const int chunks = (KP + 63) / 64 * 8;
     int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t total = user_tiles * BM * chunks;
@@ -426,8 +261,6 @@ __global__ void pack_users_kernel(const float* __restrict__ E, int64_t lde, int6
             out[j] = __ushort_as_bfloat16((unsigned short)(0x8000u | bf16_ceil_pos_bits(0.0079345703125f * enorm[u] + 1e-30f)));
     }
     size_t byte = (size_t)tile * BM * chunks * 16 + tile_byte(BM, row, ch * 8);
-    // TS mode: plain row-major rows of `chunks` 16-byte pieces (each thread later stores its row into TMEM)
-    if (row_major) byte = ((size_t)(tile * BM + row) * chunks + ch) * 16;
     *reinterpret_cast<uint4*>(reinterpret_cast<unsigned char*>(Ap) + byte) = *reinterpret_cast<const uint4*>(out);
 }
 
@@ -772,8 +605,8 @@ probe_kernel(const float* __restrict__ E, int64_t lde, const float* __restrict__
 // canonical fp32 score of (u, item at position p) is at most enorm[u] * vnorm_sorted[p] (both norms are inflated by 1.0001,
 // which also covers the rounding of the fp32 fmaf chain, <= r * 2^-24 relative).  t0[u] is the k-th best exact score among
 // the probe items -- a lower bound of the user's final k-th score -- so every position with enorm * vnorm < t0 (strictly:
-// a tie could still win on the item id) is irrelevant for u, and so are all later ones.  One block per group of `cluster`
-// user tiles (they share every item tile): cut[g] = number of item tiles the group still needs.
+// a tie could still win on the item id) is irrelevant for u, and so are all later ones.  One block per user tile:
+// cut[g] = number of item tiles the tile still needs.
 __global__ void __launch_bounds__(256)
 sweep_cut_kernel(const float* __restrict__ enorm, const float* __restrict__ t0, const float* __restrict__ vnorm_sorted,
                  int64_t m, int64_t n, int users_per_group, int32_t* __restrict__ cut) {
@@ -868,8 +701,7 @@ __device__ __forceinline__ void list_insert(ListState& ls, int k, float s, int i
 // One row's staged survivors, worked on by the whole warp: lane c takes column c of every staged 32-column chunk (sweep
 // position -> item -> seen test -> exact score), the passing ones enter the row's list through warp_list_insert.  For rows
 // whose threshold filters nothing (a user whose history covers the head of the sweep order): 16 staged chunks are up to 512
-// survivors, which the owning thread alone works off in ~0.9 M cycles (measured at C2: two such flushes keep a CTA pair busy
-// 2.4x longer than the average CTA) and the warp in 16 steps.  Same results: the list is the set of the k best under a strict
+// survivors, which the owning thread alone would work off one after the other; the warp takes 32 at a time, 16 steps.  Same results: the list is the set of the k best under a strict
 // order, whoever inserts.  Returns the number of exact scores computed by this lane.
 constexpr int COOP_MIN = 64;     // survivors in one flush from which a row is handed to the whole warp
 struct CoopArgs {                // the few kernel parameters the cooperative flush reads (passed by value: no local copy of TcParams)
@@ -909,44 +741,21 @@ __device__ __noinline__ int coop_flush_row(const CoopArgs p, const float* __rest
     return n_scored;
 }
 
-// PAIR is a template parameter: a kernel that contains cta_group::2 instructions can only be launched with an even
-// cluster size ("cluster misconfiguration" otherwise), and the 1-CTA variant keeps its issue loops free of the extra branches
-// ALLW (experimental, PB200_TC_READOUT=all): all 8 epilogue warps read EVERY tile, half of its columns each, instead of
-// the two halves taking alternate tiles: half the read-out latency per tile, twice the hand-shakes per warp.  SS mode,
-// even accumulator ring only.  The default instantiations must stay byte-identical (checked with cuobjdump).
-// SLAB: the K-slab pipeline (ranks > 61) is a separate instantiation as well: the extra slab loop and the run-time stage size
-// in the issue loop cost the K <= 64 kernel 2.7 ms of 14.0 on the full C2 sweep when they were ordinary branches.
-template <bool PAIR, bool ALLW = false, bool SLAB = false>
 __global__ void __launch_bounds__(NTHREADS, 1)
 score_topk_tc_kernel(const TcParams p) {
     extern __shared__ __align__(1024) unsigned char smem[];
     // ---- carve shared memory -------------------------------------------------------
     unsigned char* sA = smem + ((1024u - (smem_u32(smem) & 1023u)) & 1023u);     // swizzle atoms need 1024 B alignment
     unsigned char* sB = sA + p.a_bytes;
-    const uint32_t slabs = SLAB ? (uint32_t)p.slabs : 1u;
-    // pair mode: this CTA stages its half of every item tile; slab mode: one 128-byte atom (64 k) of the tile per stage
-    const uint32_t stage_bytes = PAIR ? p.b_bytes / 2 : (SLAB ? (uint32_t)(BN * 128) : p.b_bytes);
-    uint2* sStage = reinterpret_cast<uint2*>(sB + (size_t)p.stages * stage_bytes);          // [CAPS][256]
+    uint2* sStage = reinterpret_cast<uint2*>(sB + (size_t)p.stages * STAGE_BYTES);          // [CAPS][256]
     volatile uint2* sThr = reinterpret_cast<volatile uint2*>(sStage + CAPS * 256);          // [2][128] {work tag, k-th score}
     uint64_t* bars = reinterpret_cast<uint64_t*>(const_cast<uint2*>(sThr) + 256);
-    // barrier layout: full[S], empty[S], tfull[2], tempty[2], a_full, a_empty
+    // barrier layout: full[MAX_STAGES], empty[MAX_STAGES], a_full, a_empty
     const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + MAX_STAGES);
-    // accumulator barriers exist per (epilogue half, accumulator): with an odd ring (TS mode, 3 accumulators) the
-    // two halves / the two MMA warps alternate on an accumulator, and a parity wait is only unambiguous when one
-    // party waits on every phase of a barrier -- so each (half, accumulator) pair gets its own pair of barriers
-    const uint32_t bar_tfull = smem_u32(bars + 2 * MAX_STAGES), bar_tempty = smem_u32(bars + 2 * MAX_STAGES + 2 * NACC);
-    const uint32_t bar_afull = smem_u32(bars + 2 * MAX_STAGES + 4 * NACC), bar_aempty = smem_u32(bars + 2 * MAX_STAGES + 4 * NACC + 1);
-    const uint32_t bar_afull2 = smem_u32(bars + 2 * MAX_STAGES + 4 * NACC + 2);          // [2] TS mode: A tile stored in TMEM buffer b
-    const uint32_t bar_afree2 = smem_u32(bars + 2 * MAX_STAGES + 4 * NACC + 4);          // [2] TS mode: buffer b no longer used by anyone
-    // pair mode, used in the leader CTA: the peer's half of stage s landed / the peer's A tile landed (relayed by the peer)
-    const uint32_t bar_pfull = smem_u32(bars + 2 * MAX_STAGES + 4 * NACC + 6), bar_pafull = smem_u32(bars + 3 * MAX_STAGES + 4 * NACC + 6);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * MAX_STAGES + 4 * NACC + 7);
+    const uint32_t bar_afull = smem_u32(bars + 2 * MAX_STAGES), bar_aempty = smem_u32(bars + 2 * MAX_STAGES + 1);
     // flush generation of this CTA: a warp that has to work off its staged survivors bumps it, the other seven follow at
-    // their next tile.  The accumulator ring couples the warps -- while one of them rescored, the others soon waited for
-    // tiles (flat-norm input: 53 % of an epilogue warp's time) -- so they may as well rescore at the same time: 120 -> 78 ms
-    // there.  (Telling the peer CTA of the cluster too, which shares the item-tile ring: 72 ms, but the skewed full sweep
-    // went from 13.3 to 13.8 ms -- not kept.)
-    volatile uint32_t* flush_gen = tmem_slot + 1;
+    // their next tile.  The warps of a warpgroup meet at every wgmma, so they may as well rescore at the same time.
+    volatile uint32_t* flush_gen = reinterpret_cast<volatile uint32_t*>(bars + 2 * MAX_STAGES + 2);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     // tags of a previous launch may still sit in this shared memory: a stale entry that happened to carry this launch's
@@ -954,228 +763,63 @@ score_topk_tc_kernel(const TcParams p) {
     if (tid < 256) { const_cast<uint2*>(sThr)[tid] = make_uint2(0u, 0u); }
     if (tid == 0) {
         *flush_gen = 0u;
-        // pair mode: only the leader's MMA warps commit (to both CTAs); the leader's accumulator barriers collect the
-        // releases of both CTAs' epilogue warps
-        for (int s = 0; s < p.stages; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, PAIR ? 1 : p.cluster); mbar_init(bar_pfull + 8 * s, 1); }
-        for (int a = 0; a < 2 * NACC; ++a) { mbar_init(bar_tfull + 8 * a, 1); mbar_init(bar_tempty + 8 * a, (PAIR ? NEPI_WARPS : NEPI_WARPS / 2) * (ALLW ? 2 : 1)); }
-        mbar_init(bar_pafull, 1);
+        for (int s = 0; s < p.stages; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, NCONS / 32); }
         mbar_init(bar_afull, 1);
-        mbar_init(bar_aempty, 2 + NEPI_WARPS);
-        mbar_init(bar_afull2, NEPI_WARPS / 2);
-        mbar_init(bar_afull2 + 8, NEPI_WARPS / 2);
-        mbar_init(bar_afree2, 2 + NEPI_WARPS);
-        mbar_init(bar_afree2 + 8, 2 + NEPI_WARPS);
+        mbar_init(bar_aempty, NCONS / 32);
         fence_barrier_init();
         if (p.hdbg && blockIdx.x == 0) p.hdbg[5] = bar_full;     // lets a timeout report be decoded: (bar - base) / 8 = barrier index
     }
-    if (warp == 9) {
-        if (PAIR) { tmem_alloc2(smem_u32(tmem_slot), 512); tmem_relinquish2(); }
-        else { tmem_alloc(smem_u32(tmem_slot), 512); tmem_relinquish(); }
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    if (p.cluster > 1) cluster_sync_all();             // peers' barriers are initialised before anyone signals them
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t crank = p.cluster > 1 ? cluster_ctarank() : 0;
-    const uint16_t cmask = (uint16_t)((1u << p.cluster) - 1);
 
-    // a cluster walks over groups of `cluster` consecutive user tiles (same item part); CTA `crank` owns tile crank
-    const int64_t n_groups = ((p.user_tiles + p.cluster - 1) / p.cluster) * p.parts;
-    const int64_t n_clusters = gridDim.x / p.cluster, cluster_id = blockIdx.x / p.cluster;
+    const int64_t n_groups = p.user_tiles * p.parts;
+    const int64_t n_ctas = gridDim.x, cta = blockIdx.x;
     WorkItem wk;
-    const int kb = p.KP / 16;                          // MMA instructions per tile
-    const uint32_t nacc = (uint32_t)p.nacc;
-    const uint32_t aperiod = (nacc & 1) ? 2 * nacc : nacc;   // tiles between two uses of one (half, accumulator) barrier pair
-    const uint32_t a_cols = (uint32_t)p.KP / 2;        // TS: 32-bit TMEM columns of one A tile (two bf16 per column)
-    const uint32_t a_tmem0 = tmem_base + nacc * BN;    // TS: A buffers sit behind the accumulator ring
+    const uint32_t S = (uint32_t)p.stages;
+    const int KA = (p.KP + 63) / 64;                   // K slabs per item tile
 
-    if (warp == 8) {
+    if (warp == NCONS / 32) {
         // ============================ producer ======================================
         if (lane == 0) {
             uint32_t stage = 0, phase = 0, awork = 0;
-            for (int64_t wi = 0; next_work(p, wi, cluster_id, n_clusters, n_groups, wk); ++wi, ++awork) {
-                const int64_t ut = wk.g * p.cluster + crank; const int part = wk.part;
-                const int64_t t_lo = min(p.item_tiles, p.tile_first + (int64_t)part * p.tiles_per_part);
-                int64_t t_hi = min(p.item_tiles, p.tile_first + (int64_t)(part + 1) * p.tiles_per_part);
+            for (int64_t wi = 0; next_work(p, wi, cta, n_ctas, n_groups, wk); ++wi, ++awork) {
+                const int64_t t_lo = min(p.item_tiles, p.tile_first + (int64_t)wk.part * p.tiles_per_part);
+                int64_t t_hi = min(p.item_tiles, p.tile_first + (int64_t)(wk.part + 1) * p.tiles_per_part);
                 if (p.cut) t_hi = min(t_hi, max(t_lo, (int64_t)__ldg(p.cut + wk.g)));
-                if (!p.ts) {
-                    mbar_wait(bar_aempty, (awork & 1) ^ 1, p.stats, p.hdbg);
-                    mbar_arrive_expect_tx(bar_afull, p.a_bytes);
-                    bulk_g2s(smem_u32(sA), reinterpret_cast<const unsigned char*>(p.Ap) + (size_t)ut * p.a_bytes, p.a_bytes, bar_afull);
-                }
+                mbar_wait(bar_aempty, (awork & 1) ^ 1, p.stats, p.hdbg);
+                mbar_arrive_expect_tx(bar_afull, p.a_bytes);
+                bulk_g2s(smem_u32(sA), reinterpret_cast<const unsigned char*>(p.Ap) + (size_t)wk.g * p.a_bytes, p.a_bytes, bar_afull);
                 for (int64_t t = t_lo; t < t_hi; ++t) {
-                    for (uint32_t sl = 0; sl < slabs; ++sl) {
-                        // source of this stage: the whole packed tile, or its K slab `sl` (atoms are contiguous in the tile)
+                    for (int sl = 0; sl < KA; ++sl) {
+                        // K slab `sl` of item tile t (the atoms of a packed tile are contiguous)
                         const unsigned char* src = reinterpret_cast<const unsigned char*>(p.Bp) + (size_t)t * p.b_bytes +
-                                                   (size_t)sl * stage_bytes;
+                                                   (size_t)sl * STAGE_BYTES;
                         mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.stats, p.hdbg);
-                        mbar_arrive_expect_tx(bar_full + 8 * stage, stage_bytes);
-                        if (PAIR) {
-                            // rows [64 crank, 64 crank + 64) of the tile: the pair's MMA reads N/2 item rows from each CTA
-                            bulk_g2s(smem_u32(sB + (size_t)stage * stage_bytes), src + (size_t)crank * stage_bytes,
-                                     stage_bytes, bar_full + 8 * stage);
-                        } else if (p.cluster == 1) {
-                            bulk_g2s(smem_u32(sB + (size_t)stage * stage_bytes), src, stage_bytes, bar_full + 8 * stage);
-                        } else {
-                            // every CTA of the cluster fetches 1/cluster of the stage from L2 and multicasts it to all
-                            const uint32_t slice = stage_bytes / p.cluster;
-                            bulk_g2s_mc(smem_u32(sB + (size_t)stage * stage_bytes) + crank * slice, src + (size_t)crank * slice,
-                                        slice, bar_full + 8 * stage, cmask);
-                        }
-                        if (++stage == (uint32_t)p.stages) { stage = 0; phase ^= 1; }
+                        mbar_arrive_expect_tx(bar_full + 8 * stage, STAGE_BYTES);
+                        bulk_g2s(smem_u32(sB + (size_t)stage * STAGE_BYTES), src, STAGE_BYTES, bar_full + 8 * stage);
+                        if (++stage == S) { stage = 0; phase ^= 1; }
                     }
                 }
-            }
-        }
-    } else if (warp >= 9) {
-        // ============================ MMA issuers ===================================
-        // warps 9 and 10 take alternate tiles (global tile index parity); all 32 lanes run the loop
-        // (warp-uniform values), one elected lane issues each tcgen05 op
-        if (PAIR && crank != 0) {
-            // ---- peer CTA of a pair: no MMA issue here.  These two warps relay "my half of the stage landed" (and warp 9
-            // "my A tile landed") to the leader's barriers; the leader's cta_group::2 MMAs read this CTA's shared memory.
-            const uint32_t wsel = (uint32_t)(warp - 9);
-            const uint32_t S = (uint32_t)p.stages;
-            uint32_t awork = 0, g = 0, x = wsel, stage = wsel % S, phase = (wsel / S) & 1;
-            for (int64_t wi = 0; next_work(p, wi, cluster_id, n_clusters, n_groups, wk); ++wi, ++awork) {
-                const int part = wk.part;
-                const int64_t t_lo = min(p.item_tiles, p.tile_first + (int64_t)part * p.tiles_per_part);
-                int64_t t_hi = min(p.item_tiles, p.tile_first + (int64_t)(part + 1) * p.tiles_per_part);
-                if (p.cut) t_hi = min(t_hi, max(t_lo, (int64_t)__ldg(p.cut + wk.g)));
-                const uint32_t g_end = g + (uint32_t)(t_hi - t_lo);
-                if (wsel == 0) {
-                    mbar_wait(bar_afull, awork & 1, p.stats, p.hdbg);
-                    if (lane == 0) mbar_arrive_cta(bar_pafull, 0);
-                }
-                for (; x < g_end; x += 2) {
-                    mbar_wait(bar_full + 8 * stage, phase, p.stats, p.hdbg);
-                    if (lane == 0) mbar_arrive_cta(bar_pfull + 8 * stage, 0);
-                    stage += 2; if (stage >= S) { stage -= S; phase ^= 1; }
-                }
-                g = g_end;
-            }
-        } else {
-            const uint32_t wsel = (uint32_t)(warp - 9);
-            const uint32_t idesc = PAIR ? umma_idesc_bf16(2 * BM, BN) : umma_idesc_bf16(BM, BN);
-            const uint64_t adesc0 = umma_desc_sw128(smem_u32(sA));
-            const uint64_t bdesc_base = umma_desc_sw128(smem_u32(sB));
-            const uint32_t bstep = stage_bytes >> 4;               // descriptor address field is in 16-byte units
-            const uint32_t mc = p.cluster > 1 ? 1u : 0u;
-            const uint32_t S = (uint32_t)p.stages;                 // even or odd, >= 2
-            uint32_t awork = 0, g = 0;                             // g: global index of the first tile of the current work
-            // Two issuing warps alternate tiles.  In the K-slab pipeline a tile consumes `slabs` stages.  A parity wait can only
-            // tell "the next phase" from "the one before", so a warp may start waiting for slab g only when slab g - stages
-            // (the previous tenant of that stage) has LANDED.  Slabs land in order, and the warp has itself seen slab g - 1
-            // (inside a tile) or slab g - slabs - 1 (its previous tile) land: safe iff stages >= slabs + 1.  With a shorter
-            // ring (rank > ~250: the resident A tile leaves room for 3-6 stages) the first wait of a tile could fall through
-            // on a stale phase (seen as a barrier timeout at C5, rank 500): there ONE warp issues every tile (p.tok; the other
-            // only takes part in the per-work hand-shakes).  Measured alternatives: token barriers that order the two warps'
-            // waits (rank 500: 0.13 of peak instead of 0.21 with one issuer; rank 128, where no guard is needed: 59 ms instead
-            // of 42), one issuer everywhere (rank 128: 72 ms).
-            const bool single = SLAB && p.tok;
-            const uint32_t xstep = single ? 1u : 2u;
-            uint32_t x = single ? (wsel == 0 ? 0u : 0xFFFFFFF0u) : wsel;
-            uint32_t stage = wsel % S, phase = (wsel / S) & 1, acc = single ? 0u : wsel % nacc, use = single ? 0u : wsel / nacc;
-            const bool even_ring = (nacc & 1) == 0;    // then tile parity == accumulator parity and `use` counts this barrier's phases
-            const bool tr = PB_TRACE(p) != nullptr && blockIdx.x == 0 && lane == 0;
-            for (int64_t wi = 0; next_work(p, wi, cluster_id, n_clusters, n_groups, wk); ++wi, ++awork) {
-                const int part = wk.part;
-                const int64_t t_lo = min(p.item_tiles, p.tile_first + (int64_t)part * p.tiles_per_part);
-                int64_t t_hi = min(p.item_tiles, p.tile_first + (int64_t)(part + 1) * p.tiles_per_part);
-                if (p.cut) t_hi = min(t_hi, max(t_lo, (int64_t)__ldg(p.cut + wk.g)));
-                const uint32_t g_end = g + (uint32_t)(t_hi - t_lo);
-                // TS: buffer b = awork % a_bufs is (re)filled once per use; its barrier phase counts those uses
-                const uint32_t abuf = p.a_bufs == 2 ? (awork & 1) : 0, ause = p.a_bufs == 2 ? (awork >> 1) : awork;
-                if (p.ts) mbar_wait(bar_afull2 + 8 * abuf, ause & 1, p.stats, p.hdbg); else mbar_wait(bar_afull, awork & 1, p.stats, p.hdbg);
-                if (PAIR) mbar_wait(bar_pafull, awork & 1, p.stats, p.hdbg);                 // the peer's A tile is in ITS shared memory
-                const uint32_t a_tmem = a_tmem0 + abuf * a_cols;
-                for (; x < g_end; x += xstep) {
-                    if (tr && x < TRACE_N) p.trace[3 * TRACE_N + x] = clock64();
-                    if (x >= nacc) {
-                        // the previous tenant of this accumulator is tile x - nacc (read by epilogue half (x - nacc) & 1)
-                        const uint32_t xp = x - nacc;
-                        const uint32_t ppar = even_ring ? ((use - 1) & 1) : ((xp / aperiod) & 1);
-                        mbar_wait(bar_tempty + 8 * (ALLW ? acc : (xp & 1) * NACC + acc), ppar, p.stats, p.hdbg);
-                    }
-                    if (tr && x < TRACE_N) p.trace[5 * TRACE_N + x] = clock64();
-                    if constexpr (SLAB) {
-                        // K-slab pipeline (ranks > 61): tile x consumes stages x*slabs .. x*slabs + slabs - 1 of the ring, the
-                        // accumulator collects all slabs (the first MMA of the tile overwrites it), A stays resident
-                        const uint32_t d = tmem_base + acc * BN;
-                        for (uint32_t sl = 0; sl < slabs; ++sl) {
-                            const uint32_t gs = x * slabs + sl, st = gs % S, ph = (gs / S) & 1u;
-                            mbar_wait(bar_full + 8 * st, ph, p.stats, p.hdbg);
-                            tc_fence_after();
-                            const int k1 = min(kb, (int)(4 * sl + 4));
-                            for (int ks = (int)(4 * sl); ks < k1; ++ks)
-                                tc_mma_bf16_elect(d, adesc0 + (uint64_t)(sl * (BM * 128 / 16) + (uint32_t)(ks & 3) * 2),
-                                                  bdesc_base + (uint64_t)(st * bstep + (uint32_t)(ks & 3) * 2), idesc, ks > 0 ? 1u : 0u);
-                            if (p.cluster == 1) tc_commit_elect(bar_empty + 8 * st); else tc_commit_mc_elect(bar_empty + 8 * st, cmask);
-                        }
-                        tc_commit_elect(bar_tfull + 8 * (ALLW ? acc : (x & 1) * NACC + acc));
-                        acc += xstep; if (acc >= nacc) { acc -= nacc; ++use; }
-                        continue;
-                    }
-                    mbar_wait(bar_full + 8 * stage, phase, p.stats, p.hdbg);
-                    if (tr && x < TRACE_N) p.trace[4 * TRACE_N + x] = clock64();
-                    if (PAIR) mbar_wait(bar_pfull + 8 * stage, phase, p.stats, p.hdbg);      // ... and the peer's half of the tile
-                    tc_fence_after();
-                    if (tr && x < TRACE_N) p.trace[x] = clock64();
-                    const uint32_t bar_acc = bar_tfull + 8 * (ALLW ? acc : (x & 1) * NACC + acc);
-                    const uint64_t bdesc0 = bdesc_base + (uint64_t)(stage * bstep);
-                    const uint32_t d = tmem_base + acc * BN;
-                    if (PAIR && kb == 4) {
-                        tc_tile4_pair_elect(d, adesc0, bdesc0, idesc, bar_empty + 8 * stage, bar_acc);
-                    } else if (PAIR) {               // K padded to 16, 32 or 48 (rank <= 45)
-                        for (int ks = 0; ks < kb; ++ks) tc_mma_bf16_pair_elect(d, adesc0 + 2 * ks, bdesc0 + 2 * ks, idesc, ks > 0 ? 1u : 0u);
-                        tc_commit_pair_elect(bar_empty + 8 * stage);
-                        tc_commit_pair_elect(bar_acc);
-                    } else if (kb == 4 && (PB_DBG(p) & 3) != 2) {  // K padded to one 128-byte atom (rank <= 61): the common case
-                        if (p.ts) tc_tile4_ts_elect(d, a_tmem, bdesc0, idesc, bar_empty + 8 * stage, bar_acc, mc, cmask);
-                        else tc_tile4_elect(d, adesc0, bdesc0, idesc, bar_empty + 8 * stage, bar_acc, mc, cmask);
-                    } else {
-                        if ((PB_DBG(p) & 3) != 2) {
-                            for (int ks = 0; ks < kb; ++ks) {
-                                // k-step ks covers k = 16*ks .. +15: atom ks/4, 32 bytes per step inside the atom
-                                const uint32_t ao = (uint32_t)(ks >> 2) * (BM * 128 / 16) + (uint32_t)(ks & 3) * 2;
-                                const uint32_t bo = (uint32_t)(ks >> 2) * (BN * 128 / 16) + (uint32_t)(ks & 3) * 2;
-                                if (p.ts) tc_mma_bf16_ts_elect(d, a_tmem + 8 * ks, bdesc0 + bo, idesc, ks > 0 ? 1u : 0u);
-                                else tc_mma_bf16_elect(d, adesc0 + ao, bdesc0 + bo, idesc, ks > 0 ? 1u : 0u);
-                            }
-                        }
-                        // smem stage reusable once these MMAs retire -- in EVERY CTA of the cluster (peers write into it)
-                        if (p.cluster == 1) tc_commit_elect(bar_empty + 8 * stage); else tc_commit_mc_elect(bar_empty + 8 * stage, cmask);
-                        tc_commit_elect(bar_acc);              // accumulator ready for the epilogue
-                    }
-                    stage += 2; if (stage >= S) { stage -= S; phase ^= 1; }
-                    acc += 2; if (acc >= nacc) { acc -= nacc; ++use; }
-                }
-                // this warp's MMAs no longer read the A tile
-                if (PAIR) tc_commit_pair_elect(bar_aempty);
-                else if (p.ts) tc_commit_elect(bar_afree2 + 8 * abuf);
-                else tc_commit_elect(bar_aempty);
-                g = g_end;
             }
         }
     } else {
-        // ============================ epilogue ======================================
-        const int q = warp & 3, h = warp >> 2;                 // TMEM lane quarter, column half
-        const int row = 32 * q + lane;
-        const int etid = warp * 32 + lane;                     // 0..255
+        // ============================ consumers =====================================
+        // Warpgroup wg multiplies users [64 wg, 64 wg + 64) of the tile.  In the accumulator layout a quad of lanes holds
+        // two users (rows r and r + 8) and all 128 items between them; lane q of the quad owns row r + 8 (q >> 1) and the
+        // item half h = q & 1 (32-column chunks 2h, 2h + 1).  Each (user, half) keeps its own candidate list.
+        const int wg = warp >> 2;
+        const int q = lane & 3, h = q & 1;
+        const int row = wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * (q >> 1);
+        const int etid = tid;                                  // 0..255 = 32 warp + lane
         // byte offset of this row's threshold pair inside the packed A tile
         const uint32_t thr_off = (uint32_t)tile_byte(BM, row, p.rs);
         const bool vec_ok = ((p.lde | p.ldv) % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.E) | reinterpret_cast<uintptr_t>(p.V)) % 16 == 0);
-        const int r4 = p.r / 4;
-        uint32_t awork = 0, gcount = 0;          // gcount: tiles issued so far by this CTA (same count in the MMA warp)
-        const bool even_ring = (nacc & 1) == 0;
+        const uint64_t adesc0 = gmma_desc_sw128(smem_u32(sA) + (uint32_t)wg * 64 * 128);
+        const uint64_t bdesc0 = gmma_desc_sw128(smem_u32(sB));
+        uint32_t awork = 0, gslab = 0;           // gslab: ring stages consumed so far (the producer fills them in this order)
         unsigned long long n_rescored = 0, n_swept = 0;
         uint32_t my_gen = 0;
-        const bool prof = PB_PROF(p) != nullptr && etid == 0 && h == 0;
-        long long pf_t0 = prof ? clock64() : 0, pf_flush = 0, pf_tfull = 0, pf_afull = 0, pf_items = 0, pf_tiles = 0, pf_surv = 0, pf_maxflush = 0, pf_setup = 0, pf_body = 0, pf_first = 0;
-        for (int64_t wi = 0; next_work(p, wi, cluster_id, n_clusters, n_groups, wk); ++wi, ++awork) {
-            const long long pf_top = prof ? clock64() : 0;
-            const int64_t ut = wk.g * p.cluster + crank; const int part = wk.part;
+        for (int64_t wi = 0; next_work(p, wi, cta, n_ctas, n_groups, wk); ++wi, ++awork) {
+            const int64_t ut = wk.g; const int part = wk.part;
             const int64_t t_lo = min(p.item_tiles, p.tile_first + (int64_t)part * p.tiles_per_part);
             int64_t t_hi = min(p.item_tiles, p.tile_first + (int64_t)(part + 1) * p.tiles_per_part);
             if (p.cut) t_hi = min(t_hi, max(t_lo, (int64_t)__ldg(p.cut + wk.g)));
@@ -1192,51 +836,12 @@ score_topk_tc_kernel(const TcParams p) {
             if (live && p.seen_indptr) { sb = p.seen_indptr[u]; se = p.seen_indptr[u + 1]; }
             const uint32_t* head = (live && p.headbits) ? p.headbits + u * HEAD_WORDS : nullptr;
             int scount = 0;
-            uint32_t cur_packed = live ? pack_threshold(t_row) : 0x00007F7Fu;     // this row's threshold pair as the MMA sees it
-            const uint32_t abuf = p.a_bufs == 2 ? (awork & 1) : 0, ause = p.a_bufs == 2 ? (awork >> 1) : awork;
-            const uint32_t lane_base = (uint32_t)(32 * q) << 16;
-            const uint32_t a_tmem = a_tmem0 + abuf * a_cols;
-            if (p.ts) {
-                // warps 0-3 (one per TMEM lane quarter) store A tiles: thread = row, two bf16 per 32-bit column
-                auto store_a_tile = [&](int64_t ut_x, uint32_t buf, uint32_t use) {
-                    mbar_wait(bar_afree2 + 8 * buf, (use & 1) ^ 1, p.stats, p.hdbg);      // previous tenant (MMAs + all epilogue warps) is gone
-                    tc_fence_after();
-                    const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(p.Ap) +
-                                                                      (size_t)(ut_x * BM + row) * ((size_t)((p.KP + 63) / 64) * 128));
-                    for (int c = 0; c < kb; ++c) {
-                        const uint4 x0 = __ldg(src + 2 * c), x1 = __ldg(src + 2 * c + 1);
-                        const uint32_t v8[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-                        tmem_st8(lane_base + a_tmem0 + buf * a_cols + 8 * c, v8);
-                    }
-                    tmem_wait_st();
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(bar_afull2 + 8 * buf);
-                };
-                if (h == 0) {
-                    if (p.a_bufs == 2) {
-                        if (awork == 0) store_a_tile(ut, 0, 0);
-                        WorkItem wn;                                              // this CTA's next work: prefetch its A tile
-                        if (next_work(p, wi + 1, cluster_id, n_clusters, n_groups, wn)) store_a_tile(wn.g * p.cluster + crank, abuf ^ 1, (awork + 1) >> 1);
-                    } else {
-                        store_a_tile(ut, 0, awork);
-                    }
-                }
-                mbar_wait(bar_afull2 + 8 * abuf, ause & 1, p.stats, p.hdbg);              // A tile (and its threshold column) is in TMEM
-                tc_fence_after();
-            } else {
-                const long long c0 = prof ? clock64() : 0;
-                if (prof) pf_setup += c0 - pf_top;
-                mbar_wait(bar_afull, awork & 1, p.stats, p.hdbg);                          // A tile (and its threshold slots) landed
-                if (prof) pf_afull += clock64() - c0;
-            }
+            mbar_wait(bar_afull, awork & 1, p.stats, p.hdbg);                              // A tile (and its threshold slots) landed
 
             auto flush = [&]() {
-                const long long fc0 = prof ? clock64() : 0;
                 {
                     int nsurv = 0;
                     for (int e = 0; e < scount; ++e) nsurv += __popc(sStage[e * 256 + etid].y);
-                    if (prof) pf_surv += nsurv;
                     uint32_t big = __ballot_sync(0xffffffffu, live && nsurv >= COOP_MIN);
                     if (big) {
                         __syncwarp();                              // the owners' list entries are visible to the warp
@@ -1247,6 +852,7 @@ score_topk_tc_kernel(const TcParams p) {
                             const int64_t sb_s = __shfl_sync(0xffffffffu, sb, src), se_s = __shfl_sync(0xffffffffu, se, src);
                             const int n_s = __shfl_sync(0xffffffffu, scount, src);
                             const float t_s = __shfl_sync(0xffffffffu, t_row, src);
+                            const int h_s = __shfl_sync(0xffffffffu, h, src);
                             int cnt_s = __shfl_sync(0xffffffffu, ls.cnt, src);
                             float kth_s = __shfl_sync(0xffffffffu, ls.kth, src);
                             CoopArgs ca;
@@ -1254,7 +860,7 @@ score_topk_tc_kernel(const TcParams p) {
                             ca.seen_offset = p.seen_offset; ca.n = p.n; ca.r = p.r; ca.k = p.k;
                             n_rescored += (unsigned long long)coop_flush_row(
                                 ca, p.E + u_s * p.lde, sStage + (etid - lane + src), n_s, t_lo, sb_s, se_s, p.headbits != nullptr,
-                                p.lists + ((int64_t)(part * 2 + h) * p.m + u_s) * p.k, t_s, vec_ok, lane, cnt_s, kth_s);
+                                p.lists + ((int64_t)(part * 2 + h_s) * p.m + u_s) * p.k, t_s, vec_ok, lane, cnt_s, kth_s);
                             if (lane == src) { ls.cnt = cnt_s; ls.kth = kth_s; scount = 0; }
                         } while (big);
                         __syncwarp();
@@ -1270,9 +876,7 @@ score_topk_tc_kernel(const TcParams p) {
                         const int64_t pos = base + c;
                         if (pos >= p.n) continue;
                         const int64_t item = __ldg(p.perm + pos);          // sweep position -> item id
-                        // positions inside the head were masked by the bitmap already.  (Scoring first and looking only the
-                        // passing survivors up, and a 16-way lookup with 2 dependent round trips instead of 7, were both measured
-                        // slower: flat-norm case 135 / 139 ms against 123 ms -- the upper levels of the binary search hit in L1.)
+                        // positions inside the head were masked by the bitmap already
                         if (sb < se && (head == nullptr || pos >= HEAD_TILES * BN) &&
                             seen_lookup(p.seen_indices, sb, se, (int)(item + p.seen_offset))) continue;
                         const float* vrow = p.V + item * p.ldv;
@@ -1294,102 +898,80 @@ score_topk_tc_kernel(const TcParams p) {
                 // is the k-th score of k real unseen items of this user, hence a valid lower bound
                 const float other = (otag == awork + 1) ? oval : -CUDART_INF_F;
                 t_row = fmaxf(t_row, fmaxf(ls.kth, other));
-                const bool changed = live && t_row > t_written;
-                if (changed) { cur_packed = pack_threshold(t_row); t_written = t_row; }
-                if (!p.ts) {
-                    if (changed) {
-                        *reinterpret_cast<volatile uint32_t*>(sA + thr_off) = cur_packed;
-                        fence_proxy_async();                   // make the generic-proxy store visible to the MMA reads
-                    }
-                } else {
-                    __syncwarp();
-                    if (__any_sync(0xffffffffu, changed) && !(PB_DBG(p) & 8)) {
-                        // every lane rewrites its own row's threshold column (unchanged rows store the same value);
-                        // the other half-warp of this row may overwrite it with its own valid lower bound
-                        tmem_st1(lane_base + a_tmem + (uint32_t)(p.rs / 2), cur_packed);
-                    }
+                if (live && t_row > t_written) {
+                    // both halves of a row may write: each writes a valid lower bound
+                    *reinterpret_cast<volatile uint32_t*>(sA + thr_off) = pack_threshold(t_row);
+                    t_written = t_row;
+                    fence_proxy_async();                       // make the generic-proxy store visible to the wgmma reads
                 }
-                if (prof) { const long long d = clock64() - fc0; pf_flush += d; pf_maxflush = max(pf_maxflush, d); }
             };
 
             const int ntiles = (int)(t_hi - t_lo);
-            // warp half h takes the tiles whose running index has parity h (accumulators h, h+2 of the ring)
-            for (int j = ALLW ? 0 : (int)((gcount & 1u) != (uint32_t)h); j < ntiles; j += ALLW ? 1 : 2) {
-                const uint32_t g = gcount + (uint32_t)j;
-                const uint32_t acc = even_ring ? (g & (nacc - 1)) : (g % nacc);          // nacc is 4 (SS) or 3 (TS)
-                const uint32_t aphase = even_ring ? ((g >> 2) & 1) : ((g / aperiod) & 1);
+            for (int j = 0; j < ntiles; ++j) {
                 const int64_t t = t_lo + j;
-                const uint32_t bar_rel = bar_tempty + 8 * (ALLW ? acc : h * NACC + acc);
-                const long long c1 = prof ? clock64() : 0;
-                mbar_wait(bar_tfull + 8 * (ALLW ? acc : h * NACC + acc), aphase, p.stats, p.hdbg);
-                const long long c2 = prof ? clock64() : 0;
-                if (prof) { pf_tfull += c2 - c1; if (j < 2) pf_first += c2 - c1; }
-                if (PB_TRACE(p) && blockIdx.x == 0 && q == 0 && lane == 0 && g < TRACE_N) p.trace[TRACE_N + g] = clock64();
-                tc_fence_after();
-                const uint32_t tbase = tmem_base + ((uint32_t)(32 * q) << 16) + acc * BN;
-                // seen items in the head of the sweep order are masked here, before they become candidates
-                uint4 hb = make_uint4(0u, 0u, 0u, 0u);
-                if (head && t < HEAD_TILES) hb = __ldg(reinterpret_cast<const uint4*>(head + (int)t * (BN / 32)));
-                const uint32_t code = (uint32_t)j << 2;
-                uint32_t va[32], vb[32];
-                // one funnel shift per accumulator packs the sign bits (sign set <=> candidate).  An OR-tree pre-test (16 LOP3 per
-                // 32 accumulators, per-column masks only when some sign is set) was measured SLOWER: 16.2 vs 14.0 ms on the full
-                // C2 sweep (profiles/README.md, r2) -- the read-out is bound by the TMEM read rate, not by the ALU pipe.
-#define PB_SIGNS(V, HB, C)                                                                         \
-                {                                                                                  \
-                    uint32_t mask = 0;                                                             \
-                    _Pragma("unroll") for (int i = 0; i < 32; ++i) mask = __funnelshift_l(V[i], mask, 1); \
-                    mask &= ~(HB);                                                                 \
-                    if (mask && live && (PB_DBG(p) & 3) != 3) { sStage[scount * 256 + etid] = make_uint2(code | (C), mask); ++scount; } \
-                }
-                if ((PB_DBG(p) & 3) == 1) {
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) { if (PAIR) mbar_arrive_cta_relaxed(bar_rel, 0); else mbar_arrive(bar_rel); }
-                    continue;
-                }
-                if constexpr (ALLW) {
-                    // this half reads columns [64 h, 64 h + 64) of EVERY tile
-                    tmem_ld32(tbase + 64 * h, va);
-                    tmem_ld32(tbase + 64 * h + 32, vb);
-                    tmem_wait_ld();
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) { if (PAIR) mbar_arrive_cta_relaxed(bar_rel, 0); else mbar_arrive(bar_rel); }
-                    if (PB_TRACE(p) && blockIdx.x == 0 && q == 0 && lane == 0 && g < TRACE_N) p.trace[2 * TRACE_N + g] = clock64();
-                    PB_SIGNS(va, (h ? hb.z : hb.x), (uint32_t)(2 * h))
-                    PB_SIGNS(vb, (h ? hb.w : hb.y), (uint32_t)(2 * h + 1))
-                    {
-                    const uint32_t gen = *flush_gen;
-                    const bool need = __any_sync(0xffffffffu, scount > CAPS - 4 || (scount >= 4 && t_row == -CUDART_INF_F));
-                    if (need || gen != my_gen) {
-                        if (need && gen == my_gen && lane == 0) atomicAdd(const_cast<uint32_t*>(flush_gen), 1u);
-                        flush();
-                        my_gen = *flush_gen;
+                // ---- D = A_wg B_t^T over the K slabs of the tile; a stage goes back to the producer when its MMAs retired
+                float d[64];
+#pragma unroll
+                for (int i = 0; i < 64; ++i) d[i] = 0.f;
+                uint32_t prev = 0;
+                for (int sl = 0; sl < KA; ++sl) {
+                    const uint32_t st = gslab % S, ph = (gslab / S) & 1u;
+                    ++gslab;
+                    mbar_wait(bar_full + 8 * st, ph, p.stats, p.hdbg);
+                    wg_fence_acc(d);
+                    wg_fence();
+                    // all four K steps of the slab: the packed atoms are zero beyond KP, and a wgmma under a data-dependent
+                    // branch makes ptxas serialize every wgmma of the kernel (C7520)
+#pragma unroll
+                    for (int ks = 0; ks < 4; ++ks)
+                        wgmma_m64n128k16(d, adesc0 + (uint64_t)((uint32_t)sl * (BM * 128 / 16) + (uint32_t)ks * 2),
+                                         bdesc0 + (uint64_t)(st * (STAGE_BYTES / 16) + (uint32_t)ks * 2), (sl | ks) != 0);
+                    wg_commit();
+                    wg_fence_acc(d);
+                    if (sl > 0) {
+                        wg_wait<1>();
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
                     }
+                    prev = st;
                 }
-                    continue;
-                }
-                tmem_ld32(tbase, va);
-                tmem_ld32(tbase + 32, vb);
-                tmem_wait_ld();
-                PB_SIGNS(va, hb.x, 0u)
-                tmem_ld32(tbase + 64, va);              // in flight while the second chunk's signs are extracted
-                PB_SIGNS(vb, hb.y, 1u)
-                tmem_ld32(tbase + 96, vb);
-                tmem_wait_ld();
-                tc_fence_before();
+                wg_wait<0>();
+                wg_fence_acc(d);
                 __syncwarp();
-                // accumulator fully read: back to the MMA warps (pair mode: they live in the leader CTA)
-                if (lane == 0) { if (PAIR) mbar_arrive_cta_relaxed(bar_rel, 0); else mbar_arrive(bar_rel); }
-                if (PB_TRACE(p) && blockIdx.x == 0 && q == 0 && lane == 0 && g < TRACE_N) p.trace[2 * TRACE_N + g] = clock64();
-                PB_SIGNS(va, hb.z, 2u)
-                PB_SIGNS(vb, hb.w, 3u)
-#undef PB_SIGNS
-                if (prof) pf_body += clock64() - c2;
+                if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+
+                // ---- sign bits -> per-row candidate masks.  Word (a, c): row r + 8a, chunk c (columns 32c .. 32c + 31),
+                // column 32c + x <-> bit 31 - x; this lane contributes columns 8i + 2q + b, the quad ORs its four parts.
+                uint32_t w[2][4];
+#pragma unroll
+                for (int a = 0; a < 2; ++a)
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) {
+                        uint32_t mk = 0;
+#pragma unroll
+                        for (int i = 0; i < 4; ++i)
+#pragma unroll
+                            for (int b = 0; b < 2; ++b)
+                                mk |= (__float_as_uint(d[4 * (4 * c + i) + 2 * a + b]) >> 31) << (31 - 8 * i - b);
+                        mk >>= 2 * q;
+                        mk |= __shfl_xor_sync(0xffffffffu, mk, 1);
+                        mk |= __shfl_xor_sync(0xffffffffu, mk, 2);
+                        w[a][c] = mk;
+                    }
+                const bool hi_row = (q >> 1) != 0;
+                uint32_t m0 = hi_row ? (h ? w[1][2] : w[1][0]) : (h ? w[0][2] : w[0][0]);
+                uint32_t m1 = hi_row ? (h ? w[1][3] : w[1][1]) : (h ? w[0][3] : w[0][1]);
+                // seen items in the head of the sweep order are masked here, before they become candidates
+                if (head && t < HEAD_TILES) {
+                    const uint2 hb = __ldg(reinterpret_cast<const uint2*>(head + (int)t * (BN / 32) + 2 * h));
+                    m0 &= ~hb.x; m1 &= ~hb.y;
+                }
+                const uint32_t code = (uint32_t)j << 2;
+                if (m0 && live) { sStage[scount * 256 + etid] = make_uint2(code | (uint32_t)(2 * h), m0); ++scount; }
+                if (m1 && live) { sStage[scount * 256 + etid] = make_uint2(code | (uint32_t)(2 * h + 1), m1); ++scount; }
                 {
                     const uint32_t gen = *flush_gen;
-                    const bool need = __any_sync(0xffffffffu, scount > CAPS - 4 || (scount >= 4 && t_row == -CUDART_INF_F));
+                    const bool need = __any_sync(0xffffffffu, scount > CAPS - 2 || (scount >= 4 && t_row == -CUDART_INF_F));
                     if (need || gen != my_gen) {
                         if (need && gen == my_gen && lane == 0) atomicAdd(const_cast<uint32_t*>(flush_gen), 1u);
                         flush();
@@ -1397,28 +979,15 @@ score_topk_tc_kernel(const TcParams p) {
                     }
                 }
             }
-            gcount += (uint32_t)ntiles;
             n_swept += (unsigned long long)ntiles;
-            if (prof) { ++pf_items; pf_tiles += ntiles; }
             flush();
             __syncwarp();
-            // this warp no longer touches the A tile
-            if (p.ts) { tmem_wait_st(); tc_fence_before(); __syncwarp(); if (lane == 0) mbar_arrive(bar_afree2 + 8 * abuf); }
-            else if (lane == 0) mbar_arrive(bar_aempty);
-        }
-        if (prof) {
-            long long* o = PB_PROF(p) + 16 * blockIdx.x;
-            o[0] = clock64() - pf_t0; o[1] = pf_flush; o[2] = pf_tfull; o[3] = pf_afull; o[4] = pf_items; o[5] = pf_tiles; o[6] = pf_setup; o[7] = pf_maxflush; o[8] = pf_body; o[9] = pf_first; o[10] = pf_surv;
+            if (lane == 0) mbar_arrive(bar_aempty);      // this warp no longer touches the A tile
         }
         if (p.stats && n_rescored) atomicAdd(p.stats + 1, n_rescored);
         if (p.stats && tid == 0 && n_swept) atomicAdd(p.stats + 5, n_swept);      // (user tile, item tile) products swept
     }
-    // ---- teardown ---------------------------------------------------------------------
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    if (p.cluster > 1) cluster_sync_all();             // nobody exits while peers may still multicast into it
-    if (warp == 9) { if (PAIR) tmem_dealloc2(tmem_base, 512); else tmem_dealloc(tmem_base, 512); }
 }
 
 }  // namespace
@@ -1430,40 +999,16 @@ int pb_score_tc(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int
     const int KP = ((rs + 3) + 15) / 16 * 16;         // + threshold hi/lo + margin slot
     const int KA = (KP + 63) / 64;                      // 128-byte swizzle atoms along K
     const uint32_t a_bytes = BM * KA * 128, b_bytes = BN * KA * 128;
-    // (a second shared-memory A buffer, so that the next work item's user tile loads during this one's sweep, was measured:
-    //  no gain, 1.99 vs 1.99 ms on the cut C2 sweep -- not kept)
-    const size_t fixed = (size_t)a_bytes + CAPS * 256 * sizeof(uint2) + 256 * sizeof(uint2) + (3 * MAX_STAGES + 4 * NACC + 10) * 8 + 1024;
+    const size_t fixed = (size_t)a_bytes + CAPS * 256 * sizeof(uint2) + 256 * sizeof(uint2) + (2 * MAX_STAGES + 4) * 8 + 1024;
     int dev_smem = 0;
     PB_CUDA(ctx, cudaDeviceGetAttribute(&dev_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
     const int64_t user_tiles = ceil_div64(m, BM), item_tiles = ceil_div64(n, BN);
-    // optional: A operand in TMEM (TS form of tcgen05.mma); needs 3 accumulators + the A tile(s) in 512 columns
-    // (measured on C2: TS 16.1 ms vs SS 16.0 ms -- the TS MMAs run ~160 cycles each next to the accumulator and
-    //  epilogue TMEM traffic -- so SS stays the default; PB200_TC_MODE=ts selects the TS pipeline)
-    int ts = 0;
-    { const char* c = getenv("PB200_TC_MODE"); if (c && c[0] == 't' && c[1] == 's' && KP / 2 + 3 * BN <= 512) ts = 1; }
-    const int nacc = ts ? 3 : NACC;
-    // pipeline stages: a whole packed item tile while it is one 128-byte atom wide (K <= 64), else ONE atom (64-wide K
-    // slab) per stage with the accumulator collecting the slabs -- the A tile (KA atoms) stays resident either way
-    const int slabs = (KA >= 2 && !ts) ? KA : 1;
-    const uint32_t stage_bytes = slabs > 1 ? (uint32_t)(BN * 128) : b_bytes;
-    int stages = (int)std::min<int64_t>(MAX_STAGES, ((int64_t)dev_smem - (int64_t)fixed) / stage_bytes);
+    // the A tile (all KA atoms) stays resident; every ring stage holds one 64-wide K slab of an item tile
+    const int stages = (int)std::min<int64_t>(MAX_STAGES, ((int64_t)dev_smem - (int64_t)fixed) / STAGE_BYTES);
     if (stages < 2) {
-        ctx->err = "tcgen05 scoring kernel: rank too large for the shared-memory pipeline (use the simt kernel)";
+        ctx->err = "tensor-core scoring kernel: rank too large for the shared-memory pipeline (use the simt kernel)";
         return PB200_ENOTIMPL;
     }
-    int a_bufs = (ts && 2 * (KP / 2) + 3 * BN <= 512) ? 2 : 1;
-    { const char* c = getenv("PB200_TC_ABUFS"); if (c && atoi(c) == 1) a_bufs = 1; }
-    int cluster = 2;                                     // CTAs sharing each B tile through multicast
-    { const char* c = getenv("PB200_TC_CLUSTER"); if (c) cluster = atoi(c); }
-    if (cluster != 1 && cluster != 2 && cluster != 4) cluster = 2;
-    while (cluster > 1 && (user_tiles < cluster || (stage_bytes / cluster) % 16 != 0)) cluster >>= 1;
-    // CTA pairs (tcgen05.mma.cta_group::2): every SM reads its own A and only half of each item tile from shared memory
-    int pair = 0;
-    { const char* c = getenv("PB200_TC_PAIR"); if (c && atoi(c) == 1 && cluster == 2 && KA == 1 && !ts) pair = 1; }
-    if (pair) stages = MAX_STAGES;                      // half-size stages: all of them fit
-    int allw = 0;                                       // experimental read-out: all 8 epilogue warps on every tile
-    { const char* c = getenv("PB200_TC_READOUT"); if (c && c[0] == 'a' && !pair && !ts && (nacc & 1) == 0) allw = 1; }
-    const int64_t user_tiles_pad = ceil_div64(user_tiles, cluster) * cluster;
     // the PROBE_ITEMS largest-norm items (whole tiles only) are scored exactly by the probe kernel and form
     // each user's first candidate list; the tensor-core sweep starts behind them
     const int64_t n_probe = std::min<int64_t>(PROBE_ITEMS, (n / BN) * BN);
@@ -1478,7 +1023,7 @@ int pb_score_tc(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int
     int32_t *iota = nullptr, *perm = nullptr, *inv_perm = nullptr;
     uint32_t* headbits = nullptr;
     pb200_cand* lists = nullptr;
-    PB_TRY(sc.alloc(&Ap, (size_t)user_tiles_pad * BM * KA * 64));
+    PB_TRY(sc.alloc(&Ap, (size_t)user_tiles * BM * KA * 64));
     PB_TRY(sc.alloc(&Bp, (size_t)item_tiles * BN * KA * 64));
     PB_TRY(sc.alloc(&enorm, (size_t)m));
     PB_TRY(sc.alloc(&vnorm, (size_t)n));
@@ -1526,117 +1071,67 @@ int pb_score_tc(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int
             return PB200_ECUDA;
         }
     }
-    // 3b) how far does each group of user tiles have to sweep?  (pb200_set_prune; exact, see sweep_cut_kernel)
+    // 3b) how far does each user tile have to sweep?  (pb200_set_prune; exact, see sweep_cut_kernel)
     int32_t *cut = nullptr, *order = nullptr;
     if (ctx->prune) {
-        const int64_t groups = user_tiles_pad / cluster;
-        PB_TRY(sc.alloc(&cut, (size_t)groups));
-        sweep_cut_kernel<<<(unsigned)groups, 256, 0, ctx->stream>>>(enorm, t0, vnorm_sorted, m, n, cluster * BM, cut);
-        // longest sweeps first (next_work): one small radix sort of the group ids by their cut
-        if (groups > 2 * (int64_t)(ctx->num_sms / cluster)) {
+        PB_TRY(sc.alloc(&cut, (size_t)user_tiles));
+        sweep_cut_kernel<<<(unsigned)user_tiles, 256, 0, ctx->stream>>>(enorm, t0, vnorm_sorted, m, n, BM, cut);
+        // longest sweeps first (next_work): one small radix sort of the tile ids by their cut
+        if (user_tiles > 2 * (int64_t)ctx->num_sms) {
             int32_t *gid = nullptr, *cut_sorted = nullptr;
-            PB_TRY(sc.alloc(&gid, (size_t)groups));
-            PB_TRY(sc.alloc(&cut_sorted, (size_t)groups));
-            PB_TRY(sc.alloc(&order, (size_t)groups));
-            iota_i32_kernel<<<(unsigned)ceil_div64(groups, 256), 256, 0, ctx->stream>>>(gid, groups);
+            PB_TRY(sc.alloc(&gid, (size_t)user_tiles));
+            PB_TRY(sc.alloc(&cut_sorted, (size_t)user_tiles));
+            PB_TRY(sc.alloc(&order, (size_t)user_tiles));
+            iota_i32_kernel<<<(unsigned)ceil_div64(user_tiles, 256), 256, 0, ctx->stream>>>(gid, user_tiles);
             int end_bit = 1;
             while (end_bit < 31 && ((int64_t)1 << end_bit) <= item_tiles) ++end_bit;
             size_t temp_bytes = 0;
-            PB_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(nullptr, temp_bytes, cut, cut_sorted, gid, order, groups, 0, end_bit, ctx->stream));
+            PB_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(nullptr, temp_bytes, cut, cut_sorted, gid, order, user_tiles, 0, end_bit, ctx->stream));
             uint8_t* temp = nullptr;
             PB_TRY(sc.alloc(&temp, temp_bytes));
-            PB_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(temp, temp_bytes, cut, cut_sorted, gid, order, groups, 0, end_bit, ctx->stream));
+            PB_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(temp, temp_bytes, cut, cut_sorted, gid, order, user_tiles, 0, end_bit, ctx->stream));
         }
     }
     // 4) operand packing (user norms feed the per-pair margin)
     {
-        int64_t tot_b = item_tiles * BN * (KA * 8), tot_a = user_tiles_pad * BM * (KA * 8);
+        int64_t tot_b = item_tiles * BN * (KA * 8), tot_a = user_tiles * BM * (KA * 8);
         pack_items_kernel<<<(unsigned)ceil_div64(tot_b, 256), 256, 0, ctx->stream>>>(V, ldv, n, r, rs, KP, item_tiles, perm, vnorm_sorted, Bp);
-        pack_users_kernel<<<(unsigned)ceil_div64(tot_a, 256), 256, 0, ctx->stream>>>(E, lde, m, r, rs, KP, user_tiles_pad, enorm, t0, Ap, ts);
+        pack_users_kernel<<<(unsigned)ceil_div64(tot_a, 256), 256, 0, ctx->stream>>>(E, lde, m, r, rs, KP, user_tiles, enorm, t0, Ap);
+    }
+    if (sweep_tiles <= 0) {
+        // every item was in the probe set: only the probe list exists
+        cudaEventRecord(ctx->ev0, ctx->stream);
+        cudaEventRecord(ctx->ev1, ctx->stream);
+        *parts_out = 1;
+        *lists_out = lists + (size_t)parts * 2 * m * k;
+        PB_CUDA(ctx, cudaGetLastError());
+        return PB200_OK;
     }
     // 5) the fused tensor-core kernel
     TcParams p;
-    p.Ap = Ap; p.Bp = Bp; p.E = E; p.lde = lde; p.V = V; p.ldv = ldv; p.enorm = enorm; p.perm = perm; p.t0 = t0;
+    p.Ap = Ap; p.Bp = Bp; p.E = E; p.lde = lde; p.V = V; p.ldv = ldv; p.perm = perm; p.t0 = t0;
     p.m = m; p.n = n; p.r = r; p.KP = KP; p.rs = rs; p.k = k;
     p.user_tiles = user_tiles; p.item_tiles = item_tiles; p.parts = parts; p.tiles_per_part = tiles_per_part;
     p.tile_first = tile_first;
     p.seen_indptr = seen_indptr; p.seen_indices = seen_indices; p.seen_offset = seen_offset;
-    p.lists = lists; p.stages = stages; p.slabs = slabs; p.tok = (slabs > 1 && stages < slabs + 1) ? 1 : 0; p.a_bytes = a_bytes; p.b_bytes = b_bytes; p.headbits = headbits; p.cut = cut; p.order = order;
-    p.dbg = 0;
-#ifdef PB200_DEVEL
-    { const char* d = getenv("PB200_TC_DEBUG"); p.dbg = d ? atoi(d) : 0; }
-#endif
+    p.lists = lists; p.stages = stages; p.a_bytes = a_bytes; p.b_bytes = b_bytes;
+    p.cut = cut; p.order = order; p.headbits = headbits;
     p.stats = reinterpret_cast<unsigned long long*>(ctx->d_stats);
-    p.trace = nullptr;
-    p.prof = nullptr;
     p.hdbg = nullptr;
     if (ctx->h_dbg) {
         unsigned long long* dptr = nullptr;
-        if (cudaHostGetDevicePointer(&dptr, ctx->h_dbg, 0) == cudaSuccess) {
-            p.hdbg = dptr;
-        }
+        if (cudaHostGetDevicePointer(&dptr, ctx->h_dbg, 0) == cudaSuccess) p.hdbg = dptr;
     }
-#ifdef PB200_DEVEL
-    if (getenv("PB200_TC_PROF")) { PB_TRY(sc.alloc(&p.prof, (size_t)16 * 256)); PB_CUDA(ctx, cudaMemsetAsync(p.prof, 0, sizeof(long long) * 16 * 256, ctx->stream)); }
-    if (getenv("PB200_TC_TRACE")) { PB_TRY(sc.alloc(&p.trace, (size_t)6 * TRACE_N)); PB_CUDA(ctx, cudaMemsetAsync(p.trace, 0, sizeof(long long) * 6 * TRACE_N, ctx->stream)); }
-#endif
-    const size_t smem_bytes = fixed + (size_t)stages * (pair ? b_bytes / 2 : stage_bytes);
-    if (pair) PB_CUDA(ctx, cudaFuncSetAttribute(score_topk_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    else if (slabs > 1) PB_CUDA(ctx, cudaFuncSetAttribute(score_topk_tc_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    else if (allw) PB_CUDA(ctx, cudaFuncSetAttribute(score_topk_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    else PB_CUDA(ctx, cudaFuncSetAttribute(score_topk_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    p.cluster = cluster; p.pair = pair;
-    p.ts = ts; p.nacc = nacc; p.a_bufs = a_bufs;
-    const int64_t n_groups = (user_tiles_pad / cluster) * parts;
-    const unsigned grid = (unsigned)(std::min<int64_t>(n_groups, ctx->num_sms / cluster) * cluster);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = smem_bytes; cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cluster; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
+    const size_t smem_bytes = fixed + (size_t)stages * STAGE_BYTES;
+    PB_CUDA(ctx, cudaFuncSetAttribute(score_topk_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    const int64_t n_groups = user_tiles * parts;
+    const unsigned grid = (unsigned)std::min<int64_t>(n_groups, ctx->num_sms);
     cudaEventRecord(ctx->ev0, ctx->stream);
-    if (sweep_tiles > 0) {
-        if (pair) PB_CUDA(ctx, cudaLaunchKernelEx(&cfg, score_topk_tc_kernel<true>, p));
-        else if (slabs > 1) PB_CUDA(ctx, cudaLaunchKernelEx(&cfg, score_topk_tc_kernel<false, false, true>, p));
-        else if (allw) PB_CUDA(ctx, cudaLaunchKernelEx(&cfg, score_topk_tc_kernel<false, true>, p));
-        else PB_CUDA(ctx, cudaLaunchKernelEx(&cfg, score_topk_tc_kernel<false>, p));
-    } else {
-        // every item was in the probe set: only the probe list exists
-        *parts_out = 1;
-        *lists_out = lists + (size_t)parts * 2 * m * k;
-        cudaEventRecord(ctx->ev1, ctx->stream);
-        return PB200_OK;
-    }
+    score_topk_tc_kernel<<<grid, NTHREADS, smem_bytes, ctx->stream>>>(p);
     cudaEventRecord(ctx->ev1, ctx->stream);
-#ifdef PB200_DEVEL
-    if (p.prof) {
-        std::vector<long long> h(16 * 256);
-        cudaMemcpyAsync(h.data(), p.prof, sizeof(long long) * 16 * 256, cudaMemcpyDeviceToHost, ctx->stream);
-        cudaStreamSynchronize(ctx->stream);
-        if (FILE* f = fopen(getenv("PB200_TC_PROF"), "a")) {
-            fprintf(f, "# cta total flush wait_tfull wait_afull items tiles setup max_flush body first_waits survivors\n");
-            for (int i = 0; i < ctx->num_sms; ++i) {
-                fprintf(f, "%d", i);
-                for (int j = 0; j < 11; ++j) fprintf(f, " %lld", h[16 * i + j]);
-                fprintf(f, "\n");
-            }
-            fclose(f);
-        }
-    }
-    if (p.trace) {
-        std::vector<long long> h(6 * TRACE_N);
-        cudaMemcpyAsync(h.data(), p.trace, sizeof(long long) * 6 * TRACE_N, cudaMemcpyDeviceToHost, ctx->stream);
-        cudaStreamSynchronize(ctx->stream);
-        if (FILE* f = fopen(getenv("PB200_TC_TRACE"), "w")) {
-            for (int i = 0; i < TRACE_N; ++i) fprintf(f, "%d %lld %lld %lld %lld %lld %lld\n", i, h[i], h[TRACE_N + i], h[2 * TRACE_N + i], h[3 * TRACE_N + i], h[4 * TRACE_N + i], h[5 * TRACE_N + i]);
-            fclose(f);
-        }
-    }
-#endif
     ctx->stats[0] += (seen_indptr ? 14 : 11) + (p.cut ? 1 : 0);
     ctx->stats[2] = (uint64_t)item_tiles; ctx->stats[3] = (uint64_t)user_tiles;
-    ctx->stats[6] += (uint64_t)(user_tiles_pad * sweep_tiles);   // padded: every CTA of a cluster walks the tiles        // what [5] would grow by without the early termination
+    ctx->stats[6] += (uint64_t)(user_tiles * sweep_tiles);   // what [5] would grow by without the early termination
     PB_CUDA(ctx, cudaGetLastError());
     *parts_out = parts * 2 + 1;
     *lists_out = lists;

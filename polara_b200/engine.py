@@ -86,7 +86,7 @@ class Engine:
 
     def __init__(self, device=None):
         if not torch.cuda.is_available():
-            raise RuntimeError("polara_b200 needs a CUDA device (sm_100); there is no CPU fallback")
+            raise RuntimeError("polara_b200 needs a CUDA device (sm_90); there is no CPU fallback")
         self.lib = _StreamFollowingLib(_abi.load(), self)
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else int(device))
         with torch.cuda.device(self.device):
@@ -95,7 +95,7 @@ class Engine:
         handle = C.c_void_p()
         st = self.lib.pb200_ctx_create(self.device.index, C.c_void_p(stream), C.byref(handle))
         if st != _abi.OK:
-            raise RuntimeError("pb200_ctx_create failed with status %d (an sm_100 GPU is required)" % st)
+            raise RuntimeError("pb200_ctx_create failed with status %d (an sm_90 GPU, H100, is required)" % st)
         self.h = handle
 
     def close(self):
@@ -146,7 +146,7 @@ class Engine:
         self._check(self.lib.pb200_ctx_sync(self.h), "sync")
 
     def set_score_kernel(self, kind):
-        kind = {"simt": 0, "tcgen05": 1}.get(kind, kind)
+        kind = {"simt": 0, "tc": 1}.get(kind, kind)
         self._check(self.lib.pb200_set_score_kernel(self.h, int(kind)), "set_score_kernel")
 
     def set_spmm_kernel(self, kind):
@@ -235,9 +235,9 @@ class Engine:
         self._check(st, "spmm")
         return out
 
-    # L2 budget for the dense panel one column panel of a matrix gathers from (B200: 126 MB L2 in two halves; data
-    # read from both dies may be held twice, so well under half of it is planned for)
-    PANEL_BYTES = 40 << 20
+    # L2 budget for the dense panel one column panel of a matrix gathers from (H100: 50 MB L2 in two partitions; data
+    # read through both may be held twice, so well under half of it is planned for)
+    PANEL_BYTES = 16 << 20
 
     def panel_cols_for(self, n_cols, ell):
         """columns per panel so that the gathered slice of X (panel_cols rows of min(ell,128) floats) stays in L2;
@@ -458,7 +458,7 @@ _ENGINES = {}
 def get_engine(device=None):
     """Process-wide engine per device (created on first use)."""
     if not torch.cuda.is_available():
-        raise RuntimeError("polara_b200 needs a CUDA device (sm_100); there is no CPU fallback")
+        raise RuntimeError("polara_b200 needs a CUDA device (sm_90); there is no CPU fallback")
     idx = torch.cuda.current_device() if device is None else int(device)
     eng = _ENGINES.get(idx)
     if eng is None:

@@ -3,7 +3,7 @@
 The reference toolchain is Python, so the host side is Python too.  When the real
 ``polara`` package is importable the drop-in classes in :mod:`polara_b200.models`
 subclass *its* ``SVDModel``/``CoffeeModel`` (see ``polara_b200.models.dropin``); on a
-machine without it (the GPU box) the classes below provide the same surface
+machine without it the classes below provide the same surface
 (``build()``, ``get_recommendations()``, ``get_topk_elements()``, ``evaluate()``,
 ``recommendations``, ``rank``/``topk``/``filter_seen`` ...) with the same argument
 meaning and error behaviour, citing the reference lines they mirror.

@@ -1,8 +1,8 @@
-"""B200 drop-ins for the reference's SVDModel / ScaledSVD / CoffeeModel hot path.
+"""GPU (H100, sm_90a) drop-ins for the reference's SVDModel / ScaledSVD / CoffeeModel hot path.
 
 ``build()`` and ``get_recommendations()`` run entirely on the device through the C-ABI
 (:mod:`polara_b200.engine`); host code only converts the data model's COO arrays to CSR
-and moves buffers.  There is no CPU fallback: without the CUDA library or an sm_100
+and moves buffers.  There is no CPU fallback: without the CUDA library or an sm_90
 device every call raises.
 
 Two families of classes share the device logic (mixins below):
@@ -54,7 +54,7 @@ class _DeviceModelMixin:
     """State shared by the device models: engine handle and cached device buffers."""
 
     _engine = None
-    score_kernel = None          # None = engine default; 'simt' | 'tcgen05'
+    score_kernel = None          # None = engine default; 'simt' | 'tc'
     last_timings = None
 
     @property

@@ -8,7 +8,7 @@ Two generators:
   randomized-SVD vs ARPACK comparison, SURVEY.md §7.2).
 * :func:`popularity_csr` -- large problems in CSR form directly (Zipf item
   popularity, log-normal user degrees, ratings 1..5 from a low-rank signal);
-  used by ``bench.py`` for the BASELINE.json shapes.
+  used by ``bench.py`` for its workload shapes.
 """
 from __future__ import annotations
 

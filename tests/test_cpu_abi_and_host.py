@@ -133,7 +133,7 @@ def test_stream_schedule_covers_users_in_growing_whole_waves():
     """chunk plan of the pinned-CSR fast path: whole waves of the scoring grid, a small first chunk (its upload is the
     only exposed one) and bounded growth so that every later upload hides behind the chunk before it."""
     from polara_b200.models import stream_schedule
-    unit = 148 * 128
+    unit = 132 * 128
     for m in (1, 40_000, 250_000, 300_000, 1_000_000, 10_000_000, 12_345_678):
         b = stream_schedule(m, unit)
         assert b[0] == 0 and b[-1] == m and all(x < y for x, y in zip(b[:-1], b[1:]))

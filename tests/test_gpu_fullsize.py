@@ -1,11 +1,11 @@
-"""Parity at BASELINE.json's full C2 size (1 M users x 100 K items, 1e8 interactions, rank 50, top-10) through
+"""Parity at the full C2 size (1 M users x 100 K items, 1e8 interactions, rank 50, top-10) through
 size-independent properties -- the oracle cannot score 1e11 pairs, so the whole result is checked by invariants and a
 random sample of user rows is checked against f64 scores computed on the host:
 
   * every list: ids in range and distinct, scores non-increasing, NO seen item anywhere (checked for all 1e7 entries);
   * sampled rows: a valid top-k of the f64 scores (order contract of models.py:494-519 + 561-563), reported scores
     equal the canonical scores of the reported items;
-  * the exact fp32 SIMT kernel and the tcgen05 kernel agree bit for bit on all 1 M rows;
+  * the exact fp32 SIMT kernel and the tensor-core kernel agree bit for bit on all 1 M rows;
   * item-sharded scoring + k-way merge equals the unsharded result (all rows);
   * a second run is bit-identical (fixed summation and insertion order).
 """
@@ -42,11 +42,11 @@ def c2():
     v[:, :R] = torch.randn((N, R), generator=g, device=dev) * scale[:, None] * (0.93 ** torch.arange(R, device=dev))
     p = DeviceCSR(indptr, indices, values, (M, N))
     e = eng.spmm(p, v, ell=R)
-    eng.set_score_kernel("tcgen05")
+    eng.set_score_kernel("tc")
     ids, sc = eng.score_topk(e, v, R, K, seen=(indptr, indices), want_scores=True)
     torch.cuda.synchronize()
     yield dict(eng=eng, p=p, v=v, e=e, ids=ids, sc=sc)
-    eng.set_score_kernel("tcgen05")
+    eng.set_score_kernel("tc")
 
 
 def test_fullsize_list_invariants(c2):
@@ -92,8 +92,8 @@ def test_fullsize_kernels_agree_and_rerun_is_identical(c2):
     try:
         exact, sc_exact = eng.score_topk(e, v, R, K, seen=(p.indptr, p.indices), want_scores=True)
     finally:
-        eng.set_score_kernel("tcgen05")
-    assert torch.equal(exact, ids), "tcgen05 filter + rescoring differs from the exact fp32 kernel"
+        eng.set_score_kernel("tc")
+    assert torch.equal(exact, ids), "tensor-core filter + rescoring differs from the exact fp32 kernel"
     assert torch.equal(sc_exact, sc)
 
 

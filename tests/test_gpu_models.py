@@ -1,5 +1,5 @@
 """End-to-end parity of the device models against fixtures recorded from the REAL
-reference (tests/golden, made by oracle/make_golden.py).  B200 box only."""
+reference (tests/golden, made by oracle/make_golden.py).  H100 only."""
 import numpy as np
 import pytest
 
@@ -50,7 +50,7 @@ def test_scoring_with_reference_factors_is_exact(golden, name):
     f = model.data.fields
     model.factors = {f.userid: None, f.itemid: g["item_factors"].copy(), "singular_values": g["singular_values"]}
     model._is_ready = True
-    for kernel in ("simt", "tcgen05"):
+    for kernel in ("simt", "tc"):
         model.score_kernel = kernel
         model._recommendations = None
         recs = model.get_recommendations()
@@ -180,9 +180,9 @@ def test_streamed_fast_path_matches_plain():
 #  round-2 parity additions
 # ---------------------------------------------------------------------------------------------------------------------
 def _c1_data(warm=True):
-    """BASELINE config C1 at its real size (ML-1M shape: 6040 x 3706, 166 ratings per user ~ 1.0e6, PureSVD rank 10): the
-    same seeded generator tests/test_oracle_vs_reference.py feeds to the REAL reference; test users = the last 1208 users'
-    rows (known-user style: P = their training rows)."""
+    """Config C1 at its real size (ML-1M shape: 6040 x 3706, 166 ratings per user ~ 1.0e6, PureSVD rank 10), from the seeded
+    generator polara_b200.synth.planted_ratings; test users = the last 1208 users' rows (known-user style: P = their
+    training rows)."""
     from polara_b200.host import ArrayData
     from polara_b200.synth import planted_ratings
     u, i, r = planted_ratings(6040, 3706, 166, rank=12, seed=11)
@@ -280,12 +280,12 @@ def test_scaled_svd_rank_sweep_at_scale():
 
 def test_dropin_classes_against_the_real_reference():
     """polara_b200.models.dropin(): our device mixins grafted on the REAL polara classes, driven by a real RecommenderData
-    (needs the reference: baseline/_ref travels to the GPU box).  Same data object for both: singular values, subspace,
+    (needs the reference installed under oracle/_ref).  Same data object for both: singular values, subspace,
     lists and evaluate() hit counts vs polara's own SVDModel."""
     pd = pytest.importorskip("pandas")
     from oracle import ref_driver as rd
     if rd.reference_root() is None:
-        pytest.skip("reference not installed (baseline/_ref)")
+        pytest.skip("reference not installed (oracle/_ref)")
     rd.import_reference()
     from polara.recommender.data import RecommenderData
     from polara.recommender.models import SVDModel

@@ -1,79 +1,60 @@
-"""Oracle vs the LIVE reference on fresh seeds (build container only; skipped
-where /root/reference does not exist, e.g. on the GPU box)."""
+"""Oracle vs outputs of the reference (evfro/polara) itself, recorded by oracle/make_golden.py into
+tests/golden/reference_live.npz together with the inputs the reference's data model handed over.  CPU only."""
 import numpy as np
 import pytest
 import scipy.sparse as sps
 
 from oracle import polara_oracle as po
-from oracle.ref_shim import import_reference, reference_available
 
-pytestmark = pytest.mark.skipif(not reference_available(), reason="reference checkout absent")
+
+@pytest.fixture(scope="module")
+def ref(golden):
+    return golden("reference_live")
 
 
 @pytest.mark.parametrize("seed", [1, 2])
-def test_downvote_topk_rescale_live(seed):
-    import_reference()
-    from polara.recommender.models import RecommenderModel
-    from polara.preprocessing.matrices import rescale_matrix
+def test_downvote_topk_rescale_live(ref, seed):
     rng = np.random.default_rng(seed)
     s = rng.standard_normal((20, 50))
     rows = np.repeat(np.arange(20), 4)
     cols = np.concatenate([rng.choice(50, 4, replace=False) for _ in range(20)])
-    ref = s.copy()
-    RecommenderModel.downvote_seen_items(ref, (rows, cols))
     mine = po.downvote_seen_items(s.copy(), rows, cols)
-    np.testing.assert_array_equal(mine, ref)
+    np.testing.assert_array_equal(mine, ref["dv%d_downvoted" % seed])
     for row in range(20):
-        np.testing.assert_array_equal(po.topsort(ref[row], 6), RecommenderModel.topsort(ref[row], 6))
+        np.testing.assert_array_equal(po.topsort(mine[row], 6), ref["dv%d_topsort6" % seed][row])
     a = sps.random(40, 30, density=0.2, random_state=seed, format="csr")
-    for scaling, axis in ((0.4, 0), (0.8, 1), (1, 0)):
-        np.testing.assert_allclose(po.rescale_matrix(a, scaling, axis).toarray(),
-                                   rescale_matrix(a, scaling, axis).toarray(), rtol=1e-14)
+    for j, (scaling, axis) in enumerate(((0.4, 0), (0.8, 1), (1, 0))):
+        np.testing.assert_allclose(po.rescale_matrix(a, scaling, axis).toarray(), ref["dv%d_rescaled%d" % (seed, j)],
+                                   rtol=1e-14)
 
 
-def test_hooi_live():
-    import_reference()
-    from polara.lib.tensor import hooi
+def test_hooi_live(ref):
     rng = np.random.default_rng(3)
     shp = (40, 30, 5)
     nnz = 900
     idx = np.unique(np.stack([rng.integers(0, s, nnz) for s in shp], axis=1), axis=0).astype(np.intp)
     val = np.ones(len(idx))
-    ref = hooi(idx, val, shp, (4, 3, 2), num_iters=6, growth_tol=1e-4, seed=5)
     mine = po.hooi(idx, val, shp, (4, 3, 2), num_iters=6, growth_tol=1e-4, seed=5)
-    for a, b in zip(mine[:3], ref[:3]):
-        sv = np.linalg.svd(a.T @ b, compute_uv=False)
+    for j in range(3):
+        sv = np.linalg.svd(mine[j].T @ ref["hooi_f%d" % j], compute_uv=False)
         assert sv.min() > 1 - 1e-9
-    np.testing.assert_allclose(np.linalg.norm(mine[3]), np.linalg.norm(ref[3]), rtol=1e-10)
+    np.testing.assert_allclose(np.linalg.norm(mine[3]), np.linalg.norm(ref["hooi_core"]), rtol=1e-10)
 
 
-def test_c1_shaped_svd_model_live():
-    """BASELINE config C1 (ML-1M shape: 6040 x 3706, ~1.0e6 ratings, PureSVD rank 10, top-10) through the REAL reference
-    (RecommenderData.prepare + SVDModel.build + get_recommendations with its default chunking) against the oracle on the
-    arrays the reference's data model hands over: singular values, item-factor subspace, and every recommendation list
-    (scored with the reference's own factors: exact; with the oracle's factors: up to near-ties)."""
-    import pandas as pd
-    import_reference()
-    from polara.recommender.data import RecommenderData
-    from polara.recommender.models import SVDModel
-    from polara_b200.synth import planted_ratings
-    u, i, r = planted_ratings(6040, 3706, 166, rank=12, seed=11)
-    assert len(u) == 6040 * 166
-    data = RecommenderData(pd.DataFrame({"userid": u, "itemid": i, "rating": r}), "userid", "itemid", "rating", seed=0)
-    data.verbose = False
-    data.prepare()
-    model = SVDModel(data)
-    model.verbose = False
-    model.rank = 10
-    model.build()
-    recs = model.get_recommendations()
-    idx, val, shp = data.to_coo(tensor_mode=False)
+def test_c1_shaped_svd_model_live(ref):
+    """PureSVD rank 10, top-10 at ML-1M density (1200 x 740 users x items, 166 ratings per user) through the reference's
+    RecommenderData.prepare + SVDModel.build + get_recommendations, against the oracle on the arrays the reference's data
+    model handed over: singular values, item-factor subspace, and every recommendation list (scored with the reference's
+    own factors: exact; with the oracle's factors: up to near-ties)."""
+    idx, val, shp = ref["svd_train_idx"], ref["svd_train_val"].astype(np.float64), tuple(ref["svd_train_shape"])
+    recs = ref["svd_recs"]
     a = sps.csr_matrix((val, (idx[:, 0], idx[:, 1])), shape=shp, dtype=np.float64)
     v, s, _ = po.svd_build(a, 10)
-    np.testing.assert_allclose(s, model.factors["singular_values"], rtol=1e-9)
-    vref = model.factors[data.fields.itemid]
+    np.testing.assert_allclose(s, ref["svd_sigma"], rtol=1e-9)
+    vref = ref["svd_v"]
     assert np.linalg.svd(v.T @ vref, compute_uv=False).min() > 1 - 1e-6
-    (tu, ti, tf), tshape, _ = model._get_test_data()
+    tu, ti, tf = ref["svd_test_u"], ref["svd_test_i"], ref["svd_test_f"].astype(np.float64)
+    tshape = tuple(ref["svd_test_shape"])
     mine = po.recommend_svd(tu, ti, tf, tshape, vref, topk=10)
     assert mine.shape == recs.shape and recs.shape[1] == 10
     np.testing.assert_array_equal(mine, recs)
@@ -81,59 +62,37 @@ def test_c1_shaped_svd_model_live():
     assert (own == recs).mean() > 0.99
 
 
-def test_coffee_model_live_default_mlrank():
-    """CoffeeModel with the reference's default multilinear rank (13, 10, 2) on a 1500 x 600 x 5 tensor through the REAL
+def test_coffee_model_live_default_mlrank(ref):
+    """CoffeeModel with the reference's default multilinear rank (13, 10, 2) on a 1500 x 600 x 5 tensor through the
     reference against the oracle: HOOI from the same seed (factor subspaces, core norm) and every recommendation list
     scored with the reference's factors."""
-    import pandas as pd
-    import_reference()
-    from polara.recommender.data import RecommenderData
-    from polara.recommender.models import CoffeeModel
-    from polara_b200.synth import planted_ratings
-    u, i, r = planted_ratings(1500, 600, 40, rank=6, seed=13)
-    data = RecommenderData(pd.DataFrame({"userid": u, "itemid": i, "rating": r}), "userid", "itemid", "rating", seed=0)
-    data.verbose = False
-    data.prepare()
-    model = CoffeeModel(data)
-    model.verbose = False
-    model.seed = 3
-    model.num_iters = 8
-    model.build()
-    recs = model.get_recommendations()
-    idx, val, shp = data.to_coo(tensor_mode=True)
-    mine = po.hooi(idx.astype(np.intp), val, shp, tuple(model.mlrank), num_iters=model.num_iters,
-                   growth_tol=model.growth_tol, seed=model.seed)
-    f = data.fields
-    for got, key in zip(mine[:3], (f.userid, f.itemid, f.feedback)):
-        assert np.linalg.svd(got.T @ model.factors[key], compute_uv=False).min() > 1 - 1e-6, key
-    np.testing.assert_allclose(np.linalg.norm(mine[3]), np.linalg.norm(model.factors["core"]), rtol=1e-8)
-    (tu, ti, tf), tshape, _ = model._get_test_data()
-    lists = po.recommend_coffee(tu, ti, np.asarray(tf, dtype=np.int64), tshape, model.factors[f.itemid],
-                                model.factors[f.feedback], topk=10)
-    np.testing.assert_array_equal(lists, recs)
+    idx, val, shp = ref["cf_train_idx"].astype(np.intp), ref["cf_train_val"].astype(np.float64), tuple(ref["cf_train_shape"])
+    assert tuple(ref["cf_mlrank"]) == (13, 10, 2)
+    mine = po.hooi(idx, val, shp, tuple(int(x) for x in ref["cf_mlrank"]), num_iters=int(ref["cf_num_iters"]),
+                   growth_tol=float(ref["cf_growth_tol"]), seed=int(ref["cf_seed"]))
+    for j in range(3):
+        assert np.linalg.svd(mine[j].T @ ref["cf_f%d" % j], compute_uv=False).min() > 1 - 1e-6, j
+    np.testing.assert_allclose(np.linalg.norm(mine[3]), np.linalg.norm(ref["cf_core"]), rtol=1e-8)
+    tu, ti, tf = ref["cf_test_u"], ref["cf_test_i"], ref["cf_test_f"]
+    lists = po.recommend_coffee(tu, ti, tf, tuple(ref["cf_test_shape"]), ref["cf_f1"], ref["cf_f2"], topk=10)
+    np.testing.assert_array_equal(lists, ref["cf_recs"])
 
 
-def test_round_core_live():
+def test_round_core_live(ref):
     """CoffeeModel.round_core / _check_reduced_rank (models.py:949-980) against the oracle restatement."""
-    import_reference()
-    from polara.recommender.models import CoffeeModel
-    rng = np.random.default_rng(9)
-    core = rng.standard_normal((7, 6, 4))
-    for mode, rank in ((0, 3), (1, 6), (1, 2), (2, 1), (2, 3)):
-        rot_ref, core_ref = CoffeeModel.round_core(core, mode, rank)
+    core = ref["rc_core"]
+    np.testing.assert_array_equal(core, np.random.default_rng(9).standard_normal((7, 6, 4)))
+    for j, (mode, rank) in enumerate(((0, 3), (1, 6), (1, 2), (2, 1), (2, 3))):
         rot, new_core = po.round_core(core, mode, rank)
-        np.testing.assert_allclose(rot, rot_ref, rtol=0, atol=1e-13)
-        np.testing.assert_allclose(new_core, core_ref, rtol=0, atol=1e-13)
+        np.testing.assert_allclose(rot, ref["rc%d_rot" % j], rtol=0, atol=1e-13)
+        np.testing.assert_allclose(new_core, ref["rc%d_core" % j], rtol=0, atol=1e-13)
         assert new_core.shape[mode] == rank
 
 
 @pytest.mark.parametrize("switch_positive", [None, 4])
-def test_simple_rates_match_reference_live(switch_positive):
+def test_simple_rates_match_reference_live(ref, switch_positive):
     """evaluate(simple_rates=True) / holdout_size == 1 (models.py:451-458): hit rate, ARHR and MRR of the host mirror
     against the reference's own evaluation functions on random lists."""
-    import pandas as pd
-    import_reference()
-    from polara.recommender.evaluation import assemble_scoring_matrices, get_hr_score, get_rr_scores
     from polara_b200.host import evaluate_lists
     rng = np.random.default_rng(12)
     m, n, k = 60, 90, 10
@@ -141,12 +100,9 @@ def test_simple_rates_match_reference_live(switch_positive):
     hu = np.repeat(np.arange(m), 3)
     hi = np.concatenate([rng.choice(n, 3, replace=False) for _ in range(m)])
     hf = rng.integers(1, 6, size=len(hu)).astype(np.float64)
-    holdout = pd.DataFrame({"userid": hu, "itemid": hi, "rating": hf})
-    is_positive = None if switch_positive is None else (hf >= switch_positive)
-    data = assemble_scoring_matrices(recs, holdout, "userid", "itemid", is_positive, feedback="rating")
-    hr_ref, rr_ref = get_hr_score(data[1]), get_rr_scores(data[1])
     rel, rank = evaluate_lists(recs, hu, hi, hf, n, metric_type=["relevance", "ranking"], switch_positive=switch_positive,
                                simple_rates=True)
-    np.testing.assert_allclose(rel.hr, hr_ref.hr, rtol=1e-12)
-    np.testing.assert_allclose(rank.arhr, rr_ref.arhr, rtol=1e-12)
-    np.testing.assert_allclose(rank.mrr, rr_ref.mrr, rtol=1e-12)
+    hr_ref, arhr_ref, mrr_ref = ref["rates_%s" % switch_positive]
+    np.testing.assert_allclose(rel.hr, hr_ref, rtol=1e-12)
+    np.testing.assert_allclose(rank.arhr, arhr_ref, rtol=1e-12)
+    np.testing.assert_allclose(rank.mrr, mrr_ref, rtol=1e-12)
