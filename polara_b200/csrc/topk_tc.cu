@@ -63,8 +63,13 @@ struct TcParams {
     pb200_cand* lists;           // [parts*2][m][k]
     int stages;
     uint32_t a_bytes, b_bytes;
-    const int32_t* cut;          // [user tiles] first item tile NOT needed by any user of the tile (or null = sweep all)
-    const int32_t* order;        // [user tiles] tiles by decreasing cut (longest sweeps first), or null = natural order
+    // early termination (null = sweep all, tile row i of user tile g is user g * BM + i): users sorted by the number of
+    // item tiles they need, descending; tile row i of user tile g is user uperm[g * BM + i], which needs
+    // need_sorted[g * BM + i] item tiles, so the first row of a tile needs the most
+    const int32_t* uperm;        // [m]
+    const int32_t* need_sorted;  // [m]
+    const float* enorm;          // [m] ||e_u|| (inflated), by user id
+    const float* vnorm_sorted;   // [n] ||v|| (inflated) by sweep position
     const uint32_t* headbits;    // [m][HEAD_WORDS] seen bitmap of the head of the sweep order (or null)
     unsigned long long* stats;   // device counters
     unsigned long long* hdbg;    // pinned host memory for timeout diagnostics (or null)
@@ -76,11 +81,10 @@ struct TcParams {
 // Both roles of a CTA (producer, consumers) walk the same sequence through this function.
 struct WorkItem { int64_t g; int part; };
 __device__ __forceinline__ bool next_work(const TcParams& p, int64_t i, int64_t c, int64_t nc, int64_t n_groups, WorkItem& wk) {
-    const bool rev = p.order != nullptr && (i & 1) && (i + 1) * nc <= n_groups;
+    const bool rev = p.uperm != nullptr && (i & 1) && (i + 1) * nc <= n_groups;
     const int64_t w = i * nc + (rev ? nc - 1 - c : c);
     if (w >= n_groups) return false;
-    const int64_t gi = w / p.parts;
-    wk.g = p.order ? (int64_t)__ldg(p.order + gi) : gi;
+    wk.g = w / p.parts;                  // with early termination the user tiles come longest first already
     wk.part = (int)(w % p.parts);
     return true;
 }
@@ -227,7 +231,7 @@ __global__ void pack_items_kernel(const float* __restrict__ V, int64_t ldv, int6
 }
 
 __global__ void pack_users_kernel(const float* __restrict__ E, int64_t lde, int64_t m, int r, int rs, int KP,
-                                  int64_t user_tiles, const float* __restrict__ enorm,
+                                  int64_t user_tiles, const int32_t* __restrict__ uperm, const float* __restrict__ enorm,
                                   const float* __restrict__ t0, __nv_bfloat16* __restrict__ Ap) {
     const int chunks = (KP + 63) / 64 * 8;
     int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -236,7 +240,8 @@ __global__ void pack_users_kernel(const float* __restrict__ E, int64_t lde, int6
     int64_t tile = gid / ((int64_t)BM * chunks);
     int rem = (int)(gid % ((int64_t)BM * chunks));
     int row = rem / chunks, ch = rem % chunks;
-    int64_t u = tile * BM + row;
+    const int64_t tr = tile * BM + row;                               // tile row; padding rows (tr >= m) stay zero
+    const int64_t u = (tr < m && uperm) ? (int64_t)__ldg(uperm + tr) : tr;
     __align__(16) __nv_bfloat16 out[8];
     uint32_t thr = 0;
     if (ch == rs / 8) {
@@ -323,8 +328,33 @@ head_bitmap_kernel(const int64_t* __restrict__ seen_indptr, const int32_t* __res
     bits[u * HEAD_WORDS + lane] = sw[warp][lane];
 }
 
+// Early termination of the norm-ordered sweep (exact).  Items are visited by decreasing ||v||; by Cauchy-Schwarz the
+// canonical fp32 score of (u, item at position p) is at most enorm[u] * vnorm_sorted[p] (both norms are inflated by 1.0001,
+// which also covers the rounding of the fp32 fmaf chain, <= r * 2^-24 relative).  Any lower bound t of the user's final
+// k-th best score (t0 from the probe, later the k-th scores of the sweep's own lists) makes every position with
+// enorm * vnorm < t (strictly: a tie could still win on the item id) irrelevant for u, and all later ones too.
+// Returns the first item tile in [lo, hi] whose first position has a bound below t -- the user needs no tile from there
+// on -- or hi (t not positive and finite: no cut).  hi <= item tiles, so every probed position exists.
+__device__ __forceinline__ int first_cut_tile(float en, float t, const float* __restrict__ vnorm_sorted, int lo, int hi) {
+    if (!(t > 0.f && t < CUDART_INF_F)) return hi;
+    while (lo < hi) {                                     // bounds are non-increasing along the sweep
+        const int mid = (lo + hi) >> 1;
+        if (en * __ldg(vnorm_sorted + (int64_t)mid * BN) < t) hi = mid; else lo = mid + 1;
+    }
+    return lo;
+}
+
+// need[u] = item tiles user u needs under its bound t0[u]; used when the bounds changed after the probe (bound hook)
+__global__ void user_need_kernel(const float* __restrict__ enorm, const float* __restrict__ t0,
+                                 const float* __restrict__ vnorm_sorted, int64_t m, int item_tiles, int32_t* __restrict__ need) {
+    const int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (u < m) need[u] = first_cut_tile(__ldg(enorm + u), __ldg(t0 + u), vnorm_sorted, 0, item_tiles);
+}
+
 // Exact fp32 scores of 64 users x the PROBE_ITEMS largest-norm items; t0[u] = k-th largest unseen
 // score (a valid lower bound of the user's final k-th best score), -inf if fewer than k are unseen.
+// The probe reads every row of E anyway, so it also emits enorm[u] (the row norm, inflated like row_norm_kernel's) and,
+// when need is not null, need[u] = first_cut_tile under t0[u].
 constexpr int PTU = 64, PTI = 128, PKS = 32;
 constexpr int PNU = 2;                          // users a warp selects for at the same time (independent latency chains)
 template <int PI>
@@ -333,6 +363,7 @@ struct ProbeSmem {
     float vs[PKS][PTI + 4];
     float sc[PTU][PI + 4];                      // row stride = 4 mod 32 words: 16-byte row stores and lane-strided reads, no conflicts
     unsigned long long cand[8][PNU][32];        // per warp and user in flight: the keys that can still be among the k best
+    float t0s[PTU];
 };
 
 // order-preserving 32-bit image of a float (larger float <=> larger unsigned) and its inverse
@@ -385,7 +416,8 @@ template <int PI>
 __global__ void __launch_bounds__(256)
 probe_kernel(const float* __restrict__ E, int64_t lde, const float* __restrict__ V, int64_t ldv,
              const int32_t* __restrict__ perm, int64_t m, int64_t n_probe, int r, int k,
-             const uint32_t* __restrict__ headbits, float* __restrict__ t0, pb200_cand* __restrict__ out_list) {
+             const uint32_t* __restrict__ headbits, float* __restrict__ t0, pb200_cand* __restrict__ out_list,
+             float* __restrict__ enorm, const float* __restrict__ vnorm_sorted, int item_tiles, int32_t* __restrict__ need) {
     extern __shared__ __align__(16) unsigned char praw[];
     ProbeSmem<PI>& sm = *reinterpret_cast<ProbeSmem<PI>*>(praw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, tx = tid & 15, ty = tid >> 4;
@@ -437,6 +469,7 @@ probe_kernel(const float* __restrict__ E, int64_t lde, const float* __restrict__
     };
     if (vec) fetch(0);
     float acc[4][8];
+    float en2 = 0.f;                          // threads 0..PTU-1: squared norm of user u0 + tid
     for (int tile = 0; tile < n_tiles; ++tile) {
         const int i0 = (tile / n_ktiles) * PTI, k0 = (tile % n_ktiles) * PKS;
         if (k0 == 0) {
@@ -464,6 +497,8 @@ probe_kernel(const float* __restrict__ E, int64_t lde, const float* __restrict__
         __syncthreads();
         if (vec && tile + 1 < n_tiles) fetch(tile + 1);
         const int kmax = min(PKS, r - k0);
+        if (i0 == 0 && tid < PTU)             // the first item block walks all K tiles of E once
+            for (int kk = 0; kk < kmax; ++kk) en2 = fmaf(sm.es[kk][tid], sm.es[kk][tid], en2);
         // thread (tx, ty): users 4 ty .. 4 ty + 3, items 4 tx .. 4 tx + 3 and 64 + 4 tx .. 64 + 4 tx + 3 of the tile, so that
         // the 16 lanes of a half-warp read one contiguous 256-byte run per load
         for (int kk = 0; kk < kmax; ++kk) {
@@ -579,11 +614,11 @@ probe_kernel(const float* __restrict__ E, int64_t lde, const float* __restrict__
             if (lane < count[a] && rank < k) {
                 pb200_cand c; c.score = ord_to_float((uint32_t)(mine[a] >> 32)); c.id = (int)(0xFFFFFFFFu - (uint32_t)mine[a]);
                 out[rank] = c;
-                if (rank == k - 1) t0[u[a]] = c.score;
+                if (rank == k - 1) sm.t0s[ul + 8 * a] = c.score;
             }
             if (count[a] < k) {
                 if (lane >= count[a] && lane < k) { pb200_cand c; c.score = -CUDART_INF_F; c.id = -1; out[lane] = c; }
-                if (lane == 0) t0[u[a]] = -CUDART_INF_F;
+                if (lane == 0) sm.t0s[ul + 8 * a] = -CUDART_INF_F;
             }
         }
         __syncwarp();
@@ -596,44 +631,17 @@ probe_kernel(const float* __restrict__ E, int64_t lde, const float* __restrict__
                 const uint32_t id = ord[a][j] ? (uint32_t)__ldg(perm + lane + 32 * j) : 0u;
                 key[j] = ord[a][j] ? (((unsigned long long)ord[a][j] << 32) | (unsigned long long)(0xFFFFFFFFu - id)) : 0ull;
             }
-            probe_select_rounds<PL>(key, lane, k, out_list + u[a] * k, t0 + u[a]);
+            probe_select_rounds<PL>(key, lane, k, out_list + u[a] * k, &sm.t0s[ul + 8 * a]);
         }
     }
-}
-
-// Early termination of the norm-ordered sweep (exact).  Items are visited by decreasing ||v||; by Cauchy-Schwarz the
-// canonical fp32 score of (u, item at position p) is at most enorm[u] * vnorm_sorted[p] (both norms are inflated by 1.0001,
-// which also covers the rounding of the fp32 fmaf chain, <= r * 2^-24 relative).  t0[u] is the k-th best exact score among
-// the probe items -- a lower bound of the user's final k-th score -- so every position with enorm * vnorm < t0 (strictly:
-// a tie could still win on the item id) is irrelevant for u, and so are all later ones.  One block per user tile:
-// cut[g] = number of item tiles the tile still needs.
-__global__ void __launch_bounds__(256)
-sweep_cut_kernel(const float* __restrict__ enorm, const float* __restrict__ t0, const float* __restrict__ vnorm_sorted,
-                 int64_t m, int64_t n, int users_per_group, int32_t* __restrict__ cut) {
-    __shared__ int s_max;
-    if (threadIdx.x == 0) s_max = 0;
     __syncthreads();
-    const int64_t u0 = (int64_t)blockIdx.x * users_per_group;
-    int need = 0;
-    for (int i = threadIdx.x; i < users_per_group; i += blockDim.x) {
-        const int64_t u = u0 + i;
-        if (u >= m) continue;
-        const float t = __ldg(t0 + u), en = __ldg(enorm + u);
-        int pos = (int)n;
-        if (t > 0.f && t < CUDART_INF_F) {
-            // first position whose bound falls below t (bounds are non-increasing along the sweep)
-            int lo = 0, hi = (int)n;
-            while (lo < hi) {
-                const int mid = (lo + hi) >> 1;
-                if (en * __ldg(vnorm_sorted + mid) < t) hi = mid; else lo = mid + 1;
-            }
-            pos = lo;
-        }
-        need = max(need, pos);
+    if (tid < PTU && u0 + tid < m) {
+        const int64_t uu = u0 + tid;
+        const float t = sm.t0s[tid], en = sqrtf(en2) * 1.0001f;      // tiny inflation covers the rounding of the norm itself
+        t0[uu] = t;
+        enorm[uu] = en;
+        if (need) need[uu] = first_cut_tile(en, t, vnorm_sorted, 0, item_tiles);
     }
-    atomicMax(&s_max, need);
-    __syncthreads();
-    if (threadIdx.x == 0) cut[blockIdx.x] = (s_max + BN - 1) / BN;
 }
 
 // ------------------------------------------------------------------ main kernel ---
@@ -756,11 +764,18 @@ score_topk_tc_kernel(const TcParams p) {
     // flush generation of this CTA: a warp that has to work off its staged survivors bumps it, the other seven follow at
     // their next tile.  The warps of a warpgroup meet at every wgmma, so they may as well rescore at the same time.
     volatile uint32_t* flush_gen = reinterpret_cast<volatile uint32_t*>(bars + 2 * MAX_STAGES + 2);
+    // live cut (early termination only): consumer warp w publishes {work tag, item tile from which none of its rows needs
+    // anything} in sCut[w]; the producer stops the work item's sweep once it reaches the largest of the eight.  It tells
+    // the consumers by one extra stage that carries no data and has sStop[stage] set.
+    volatile unsigned long long* sCut = reinterpret_cast<volatile unsigned long long*>(bars + 2 * MAX_STAGES + 4);   // [8]
+    volatile uint32_t* sStop = reinterpret_cast<volatile uint32_t*>(bars + 2 * MAX_STAGES + 4 + NCONS / 32);         // [MAX_STAGES]
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     // tags of a previous launch may still sit in this shared memory: a stale entry that happened to carry this launch's
-    // work tag would be taken for a valid lower bound of another user's k-th score
+    // work tag would be taken for a valid lower bound of another user's k-th score (or for another tile's cut)
     if (tid < 256) { const_cast<uint2*>(sThr)[tid] = make_uint2(0u, 0u); }
+    if (tid < NCONS / 32) sCut[tid] = 0ull;
+    if (tid < MAX_STAGES) sStop[tid] = 0u;
     if (tid == 0) {
         *flush_gen = 0u;
         for (int s = 0; s < p.stages; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, NCONS / 32); }
@@ -784,16 +799,36 @@ score_topk_tc_kernel(const TcParams p) {
             for (int64_t wi = 0; next_work(p, wi, cta, n_ctas, n_groups, wk); ++wi, ++awork) {
                 const int64_t t_lo = min(p.item_tiles, p.tile_first + (int64_t)wk.part * p.tiles_per_part);
                 int64_t t_hi = min(p.item_tiles, p.tile_first + (int64_t)(wk.part + 1) * p.tiles_per_part);
-                if (p.cut) t_hi = min(t_hi, max(t_lo, (int64_t)__ldg(p.cut + wk.g)));
+                if (p.need_sorted) t_hi = min(t_hi, max(t_lo, (int64_t)__ldg(p.need_sorted + wk.g * BM)));
                 mbar_wait(bar_aempty, (awork & 1) ^ 1, p.stats, p.hdbg);
                 mbar_arrive_expect_tx(bar_afull, p.a_bytes);
                 bulk_g2s(smem_u32(sA), reinterpret_cast<const unsigned char*>(p.Ap) + (size_t)wk.g * p.a_bytes, p.a_bytes, bar_afull);
                 for (int64_t t = t_lo; t < t_hi; ++t) {
+                    if (p.need_sorted) {
+                        // the consumers of this work item only publish after the A tile landed, so every entry still
+                        // carries an older tag until all eight warps have spoken
+                        bool all = true;
+                        int64_t live_cut = 0;
+#pragma unroll
+                        for (int w = 0; w < NCONS / 32; ++w) {
+                            const unsigned long long e = sCut[w];
+                            all = all && (uint32_t)e == awork + 1;
+                            live_cut = max(live_cut, (int64_t)(e >> 32));
+                        }
+                        if (all && t >= live_cut) {
+                            mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.stats, p.hdbg);
+                            sStop[stage] = 1u;
+                            mbar_arrive(bar_full + 8 * stage);              // release: the flag is visible to the waiters
+                            if (++stage == S) { stage = 0; phase ^= 1; }
+                            break;
+                        }
+                    }
                     for (int sl = 0; sl < KA; ++sl) {
                         // K slab `sl` of item tile t (the atoms of a packed tile are contiguous)
                         const unsigned char* src = reinterpret_cast<const unsigned char*>(p.Bp) + (size_t)t * p.b_bytes +
                                                    (size_t)sl * STAGE_BYTES;
                         mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.stats, p.hdbg);
+                        sStop[stage] = 0u;
                         mbar_arrive_expect_tx(bar_full + 8 * stage, STAGE_BYTES);
                         bulk_g2s(smem_u32(sB + (size_t)stage * STAGE_BYTES), src, STAGE_BYTES, bar_full + 8 * stage);
                         if (++stage == S) { stage = 0; phase ^= 1; }
@@ -822,9 +857,10 @@ score_topk_tc_kernel(const TcParams p) {
             const int64_t ut = wk.g; const int part = wk.part;
             const int64_t t_lo = min(p.item_tiles, p.tile_first + (int64_t)part * p.tiles_per_part);
             int64_t t_hi = min(p.item_tiles, p.tile_first + (int64_t)(part + 1) * p.tiles_per_part);
-            if (p.cut) t_hi = min(t_hi, max(t_lo, (int64_t)__ldg(p.cut + wk.g)));
-            const int64_t u = ut * BM + row;
-            const bool live = u < p.m;
+            if (p.need_sorted) t_hi = min(t_hi, max(t_lo, (int64_t)__ldg(p.need_sorted + wk.g * BM)));
+            const int64_t tr = ut * BM + row;                              // tile row
+            const bool live = tr < p.m;
+            const int64_t u = (live && p.uperm) ? (int64_t)__ldg(p.uperm + tr) : tr;     // user id
             ListState ls;
             ls.list = p.lists + ((int64_t)(part * 2 + h) * p.m + (live ? u : 0)) * p.k;
             ls.cnt = 0; ls.kth = -CUDART_INF_F;
@@ -837,6 +873,23 @@ score_topk_tc_kernel(const TcParams p) {
             const uint32_t* head = (live && p.headbits) ? p.headbits + u * HEAD_WORDS : nullptr;
             int scount = 0;
             mbar_wait(bar_afull, awork & 1, p.stats, p.hdbg);                              // A tile (and its threshold slots) landed
+            // live cut: the item tile from which this row needs nothing under t_row (first_cut_tile; 0 for padding rows),
+            // published as the maximum over the warp.  It starts at the row's cut under t0 and falls as t_row rises.
+            int cut_row = 0;
+            auto publish_cut = [&](int64_t t_next) {
+                if (live && cut_row > t_next) {
+                    // search only when the cut moves: the bound at the start of the last needed tile fell below t_row
+                    const float en = __ldg(p.enorm + u);
+                    if (en * __ldg(p.vnorm_sorted + (int64_t)(cut_row - 1) * BN) < t_row)
+                        cut_row = first_cut_tile(en, t_row, p.vnorm_sorted, (int)t_next, cut_row - 1);
+                }
+                const int wcut = __reduce_max_sync(0xffffffffu, cut_row);
+                if (lane == 0) sCut[warp] = ((unsigned long long)(uint32_t)wcut << 32) | (unsigned long long)(awork + 1);
+            };
+            if (p.need_sorted) {
+                cut_row = live ? __ldg(p.need_sorted + tr) : 0;
+                publish_cut(t_lo);
+            }
 
             auto flush = [&]() {
                 {
@@ -907,8 +960,20 @@ score_topk_tc_kernel(const TcParams p) {
             };
 
             const int ntiles = (int)(t_hi - t_lo);
-            for (int j = 0; j < ntiles; ++j) {
+            int j = 0;
+            for (; j < ntiles; ++j) {
                 const int64_t t = t_lo + j;
+                if (p.need_sorted) {
+                    // the producer may have ended the sweep here (live cut): that stage only carries the flag
+                    const uint32_t st = gslab % S, ph = (gslab / S) & 1u;
+                    mbar_wait(bar_full + 8 * st, ph, p.stats, p.hdbg);
+                    if (sStop[st]) {
+                        ++gslab;
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(bar_empty + 8 * st);
+                        break;
+                    }
+                }
                 // ---- D = A_wg B_t^T over the K slabs of the tile; a stage goes back to the producer when its MMAs retired
                 float d[64];
 #pragma unroll
@@ -976,10 +1041,11 @@ score_topk_tc_kernel(const TcParams p) {
                         if (need && gen == my_gen && lane == 0) atomicAdd(const_cast<uint32_t*>(flush_gen), 1u);
                         flush();
                         my_gen = *flush_gen;
+                        if (p.need_sorted) publish_cut(t + 1);
                     }
                 }
             }
-            n_swept += (unsigned long long)ntiles;
+            n_swept += (unsigned long long)j;
             flush();
             __syncwarp();
             if (lane == 0) mbar_arrive(bar_aempty);      // this warp no longer touches the A tile
@@ -999,7 +1065,8 @@ int pb_score_tc(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int
     const int KP = ((rs + 3) + 15) / 16 * 16;         // + threshold hi/lo + margin slot
     const int KA = (KP + 63) / 64;                      // 128-byte swizzle atoms along K
     const uint32_t a_bytes = BM * KA * 128, b_bytes = BN * KA * 128;
-    const size_t fixed = (size_t)a_bytes + CAPS * 256 * sizeof(uint2) + 256 * sizeof(uint2) + (2 * MAX_STAGES + 4) * 8 + 1024;
+    const size_t fixed = (size_t)a_bytes + CAPS * 256 * sizeof(uint2) + 256 * sizeof(uint2) + (2 * MAX_STAGES + 4) * 8 +
+                         (NCONS / 32) * 8 + MAX_STAGES * 4 + 1024;      // + live cut entries and stop flags
     int dev_smem = 0;
     PB_CUDA(ctx, cudaDeviceGetAttribute(&dev_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
     const int64_t user_tiles = ceil_div64(m, BM), item_tiles = ceil_div64(n, BN);
@@ -1033,7 +1100,7 @@ int pb_score_tc(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int
     PB_TRY(sc.alloc(&t0, (size_t)m));
     PB_TRY(sc.alloc(&lists, (size_t)(parts * 2 + 1) * m * k));          // + the probe list
 
-    // 1) item norms; sweep order = decreasing norm (stable radix sort; CUB is used for this ordering only)
+    // 1) item norms; sweep order = decreasing norm (stable radix sort; CUB is used for the two orderings only)
     row_norm_kernel<<<(unsigned)ceil_div64(n * 32, 256), 256, 0, ctx->stream>>>(V, ldv, n, r, vnorm, nullptr);
     iota_i32_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, ctx->stream>>>(iota, n);
     {
@@ -1056,12 +1123,16 @@ int pb_score_tc(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int
         head_bitmap_kernel<<<(unsigned)ceil_div64(m * 32, 256), 256, 0, ctx->stream>>>(seen_indptr, seen_indices, seen_offset,
                                                                                      inv_perm, in_head, m, n, headbits);
     }
-    // 3) exact probe pass over the largest-norm items seeds a lower bound of every user's k-th best score
-    row_norm_kernel<<<(unsigned)ceil_div64(m * 32, 256), 256, 0, ctx->stream>>>(E, lde, m, r, enorm, nullptr);
+    // 3) exact probe pass over the largest-norm items seeds a lower bound of every user's k-th best score (and
+    //    yields the user norms and, with early termination, each user's need in item tiles)
+    const bool prune = ctx->prune != 0;
+    int32_t* need = nullptr;
+    if (prune) PB_TRY(sc.alloc(&need, (size_t)m));
     {
         PB_CUDA(ctx, cudaFuncSetAttribute(probe_kernel<PROBE_ITEMS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ProbeSmem<PROBE_ITEMS>)));
         probe_kernel<PROBE_ITEMS><<<(unsigned)ceil_div64(m, PTU), 256, sizeof(ProbeSmem<PROBE_ITEMS>), ctx->stream>>>(
-            E, lde, V, ldv, perm, m, n_probe, r, k, headbits, t0, lists + (size_t)parts * 2 * m * k);
+            E, lde, V, ldv, perm, m, n_probe, r, k, headbits, t0, lists + (size_t)parts * 2 * m * k,
+            enorm, vnorm_sorted, (int)item_tiles, ctx->bound_fn ? nullptr : need);
     }
     // 3a) item-sharded job: a bound found on any shard holds for the merged lists (pb200_set_bound_hook)
     if (ctx->bound_fn) {
@@ -1070,33 +1141,31 @@ int pb_score_tc(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int
             ctx->err = "bound hook failed with status " + std::to_string(st);
             return PB200_ECUDA;
         }
+        if (prune) user_need_kernel<<<(unsigned)ceil_div64(m, 256), 256, 0, ctx->stream>>>(enorm, t0, vnorm_sorted, m, (int)item_tiles, need);
     }
-    // 3b) how far does each user tile have to sweep?  (pb200_set_prune; exact, see sweep_cut_kernel)
-    int32_t *cut = nullptr, *order = nullptr;
-    if (ctx->prune) {
-        PB_TRY(sc.alloc(&cut, (size_t)user_tiles));
-        sweep_cut_kernel<<<(unsigned)user_tiles, 256, 0, ctx->stream>>>(enorm, t0, vnorm_sorted, m, n, BM, cut);
-        // longest sweeps first (next_work): one small radix sort of the tile ids by their cut
-        if (user_tiles > 2 * (int64_t)ctx->num_sms) {
-            int32_t *gid = nullptr, *cut_sorted = nullptr;
-            PB_TRY(sc.alloc(&gid, (size_t)user_tiles));
-            PB_TRY(sc.alloc(&cut_sorted, (size_t)user_tiles));
-            PB_TRY(sc.alloc(&order, (size_t)user_tiles));
-            iota_i32_kernel<<<(unsigned)ceil_div64(user_tiles, 256), 256, 0, ctx->stream>>>(gid, user_tiles);
-            int end_bit = 1;
-            while (end_bit < 31 && ((int64_t)1 << end_bit) <= item_tiles) ++end_bit;
-            size_t temp_bytes = 0;
-            PB_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(nullptr, temp_bytes, cut, cut_sorted, gid, order, user_tiles, 0, end_bit, ctx->stream));
-            uint8_t* temp = nullptr;
-            PB_TRY(sc.alloc(&temp, temp_bytes));
-            PB_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(temp, temp_bytes, cut, cut_sorted, gid, order, user_tiles, 0, end_bit, ctx->stream));
-        }
+    // 3b) early termination (pb200_set_prune; exact, see first_cut_tile): user tiles are formed from users of similar
+    //     need, so a tile sweeps about as far as its users need rather than as far as its neediest one does.  Users
+    //     sorted by need, descending: tile rows -> users (uperm); the tiles come out longest first (next_work).
+    int32_t *uperm = nullptr, *need_sorted = nullptr;
+    if (prune) {
+        int32_t* uiota = nullptr;
+        PB_TRY(sc.alloc(&uiota, (size_t)m));
+        PB_TRY(sc.alloc(&uperm, (size_t)m));
+        PB_TRY(sc.alloc(&need_sorted, (size_t)m));
+        iota_i32_kernel<<<(unsigned)ceil_div64(m, 256), 256, 0, ctx->stream>>>(uiota, m);
+        int end_bit = 1;                                          // need is in [0, item_tiles]
+        while (end_bit < 31 && ((int64_t)1 << end_bit) <= item_tiles) ++end_bit;
+        size_t temp_bytes = 0;
+        PB_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(nullptr, temp_bytes, need, need_sorted, uiota, uperm, m, 0, end_bit, ctx->stream));
+        uint8_t* temp = nullptr;
+        PB_TRY(sc.alloc(&temp, temp_bytes));
+        PB_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(temp, temp_bytes, need, need_sorted, uiota, uperm, m, 0, end_bit, ctx->stream));
     }
     // 4) operand packing (user norms feed the per-pair margin)
     {
         int64_t tot_b = item_tiles * BN * (KA * 8), tot_a = user_tiles * BM * (KA * 8);
         pack_items_kernel<<<(unsigned)ceil_div64(tot_b, 256), 256, 0, ctx->stream>>>(V, ldv, n, r, rs, KP, item_tiles, perm, vnorm_sorted, Bp);
-        pack_users_kernel<<<(unsigned)ceil_div64(tot_a, 256), 256, 0, ctx->stream>>>(E, lde, m, r, rs, KP, user_tiles, enorm, t0, Ap);
+        pack_users_kernel<<<(unsigned)ceil_div64(tot_a, 256), 256, 0, ctx->stream>>>(E, lde, m, r, rs, KP, user_tiles, uperm, enorm, t0, Ap);
     }
     if (sweep_tiles <= 0) {
         // every item was in the probe set: only the probe list exists
@@ -1115,7 +1184,7 @@ int pb_score_tc(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int
     p.tile_first = tile_first;
     p.seen_indptr = seen_indptr; p.seen_indices = seen_indices; p.seen_offset = seen_offset;
     p.lists = lists; p.stages = stages; p.a_bytes = a_bytes; p.b_bytes = b_bytes;
-    p.cut = cut; p.order = order; p.headbits = headbits;
+    p.uperm = uperm; p.need_sorted = need_sorted; p.enorm = enorm; p.vnorm_sorted = vnorm_sorted; p.headbits = headbits;
     p.stats = reinterpret_cast<unsigned long long*>(ctx->d_stats);
     p.hdbg = nullptr;
     if (ctx->h_dbg) {
@@ -1129,7 +1198,7 @@ int pb_score_tc(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int
     cudaEventRecord(ctx->ev0, ctx->stream);
     score_topk_tc_kernel<<<grid, NTHREADS, smem_bytes, ctx->stream>>>(p);
     cudaEventRecord(ctx->ev1, ctx->stream);
-    ctx->stats[0] += (seen_indptr ? 14 : 11) + (p.cut ? 1 : 0);
+    ctx->stats[0] += (seen_indptr ? 13 : 10) + (prune ? 2 : 0) + (prune && ctx->bound_fn ? 1 : 0);
     ctx->stats[2] = (uint64_t)item_tiles; ctx->stats[3] = (uint64_t)user_tiles;
     ctx->stats[6] += (uint64_t)(user_tiles * sweep_tiles);   // what [5] would grow by without the early termination
     PB_CUDA(ctx, cudaGetLastError());
