@@ -21,19 +21,27 @@
 
 namespace {
 
+// Singular values at or below 1e-6 * sigma_1 (Gram eigenvalues at or below 1e-12 * lam_1, the cut of svqb_matrix_kernel
+// in dense.cu) are treated as zero: sigma_j = 0 and the left singular vector U = M v_j / sigma_j is a zero column instead
+// of rounding noise amplified by 1 / sigma_j (DESIGN.md §4).
+__device__ __forceinline__ bool live_sigma(const double* __restrict__ lam, int j) {
+    const double l = lam[j];
+    return l > 0.0 && l > 1e-12 * lam[0];
+}
+
 __global__ void take_columns_kernel(const double* __restrict__ vecs /*[c x c] rows=eigvecs*/, int c, int r,
                                     const double* __restrict__ lam, int scale_inv_sigma, float* __restrict__ W /*[c x r]*/) {
     int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= c * r) return;
     int i = e / r, j = e % r;
     double s = 1.0;
-    if (scale_inv_sigma) { double l = lam[j]; s = l > 0.0 ? rsqrt(l) : 0.0; }
+    if (scale_inv_sigma) s = live_sigma(lam, j) ? rsqrt(lam[j]) : 0.0;
     W[e] = (float)(vecs[(int64_t)j * c + i] * s);
 }
 
 __global__ void sqrt_leading_kernel(const double* __restrict__ lam, int r, double* __restrict__ sigma) {
     int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j < r) sigma[j] = sqrt(fmax(lam[j], 0.0));
+    if (j < r) sigma[j] = live_sigma(lam, j) ? sqrt(lam[j]) : 0.0;
 }
 
 __global__ void rows_to_float_kernel(const double* __restrict__ vecs, int c, int r, float* __restrict__ out) {
