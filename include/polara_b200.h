@@ -248,6 +248,42 @@ int pb200_merge_cands_fill(pb200_ctx* ctx, const pb200_cand* in, int parts, int6
 int pb200_gather_dot(pb200_ctx* ctx, const float* E, int64_t lde, int64_t m, const float* V, int64_t ldv, int64_t n,
                      int r, const int64_t* user_idx, const int64_t* item_idx, int64_t count, float* out);
 
+/* On-the-fly sample of unseen items, the draw of the reference's sampled evaluation when no unseen interactions were
+ * set (RandomSampleEvaluationSVDMixin.compute_random_item_scores_gen, models.py:1137-1156); replaces sample_row_wise
+ * (polara/lib/sampler.py:96-111) and the draw inside mf_random_item_scoring (sampler.py:73-93), bit for bit: per user
+ * numba's random.seed(seeds_u32[u]) (MT19937 init_genrand), prime_sampler_state over the exclusion list, then n_samples
+ * draws randrange(remaining) through the position map.
+ *   excl_indptr int64 [m+1], excl_indices int32: the exclusion list of each user.  EXCEPTION to the CSR convention
+ *       above: the lists are ORDERED, NOT NECESSARILY SORTED, and are read in the given order (priming places the
+ *       excluded items in list order, so a permuted list draws differently).  The reference forms them as scipy's
+ *       profile + holdout sum (models.py:1145-1148), whose row order is scipy's when a holdout row is unsorted.
+ *   seeds_u32 uint32 [m] (np.random.SeedSequence(data.seed).generate_state(m), models.py:1151)
+ *   out_items int64 [m x ld_out]: the first n_samples columns of each row are written, nothing else (so the ids can be
+ *       placed right after the h holdout columns of an index block).
+ * PB200_EINVAL if a user has fewer than n_samples items left (the reference's randrange raises "empty range") or an
+ * exclusion id lies outside [0, n_items).  Synchronises the stream (the check's verdict is read back). */
+int pb200_sample_unseen(pb200_ctx* ctx, int64_t m, int64_t n_items, const int64_t* excl_indptr, const int32_t* excl_indices,
+                        const uint32_t* seeds_u32, int n_samples, int64_t* out_items, int64_t ld_out);
+
+/* The sampled evaluation fused: per user the draw of pb200_sample_unseen, the scores of the h holdout items
+ * (holdout_items int64 [m x h]) and of the n_samples drawn items -- the canonical fp32 chain of pb200_gather_dot, bit
+ * identical, NaN for holdout ids out of range, which never enter a list -- and the top-k POSITIONS in the row
+ * [holdout | sampled] by (score desc, position asc): models.py:1158-1183 (compute_holdout_scores, mf_random_item_scoring,
+ * np.apply_along_axis(topsort)).  No [m x (h + n_samples)] score or index block is formed.  out_pos int64 [m x k] (-1 pads
+ * a row with fewer than k scorable entries), out_scores float32 [m x k] or NULL.  1 <= k <= h + n_samples.  Errors and
+ * synchronisation as pb200_sample_unseen. */
+int pb200_sampled_topk(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int64_t ldv, int64_t m, int64_t n,
+                       int r, const int64_t* holdout_items, int h, const int64_t* excl_indptr, const int32_t* excl_indices,
+                       const uint32_t* seeds_u32, int n_samples, int k, int64_t* out_pos, float* out_scores);
+
+/* Position-map placement of the two sampler entries: a user whose map (2 * |exclusion| + n_samples entries at most, at a
+ * load factor <= 2/3) fits in `slots` 8-byte slots runs with the map in shared memory, the others with it in global
+ * memory.  0..6144, default 3072; 0 puts every user on the global-memory path.  Results do not depend on it. */
+int pb200_set_sampler_map_slots(pb200_ctx* ctx, int slots);
+/* the last sampler call (host array of 4 uint64): [0] users on the shared-memory map path, [1] users on the global-memory
+ * map path, [2] map slots per warp on the global path, [3] kernels launched. */
+int pb200_sampler_stats(pb200_ctx* ctx, uint64_t* out4_host);
+
 /* Dense scores S [m x lds] = E V^T for a handful of users (the single-user path of
  * models.py:277-293 expects a dense score row). */
 int pb200_score_dense(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int64_t ldv,

@@ -26,6 +26,8 @@ struct pb200_ctx {
     void* reduce_user = nullptr;
     pb200_reduce_fn bound_fn = nullptr;         // item-sharded scoring: elementwise MAX of the seed bounds over the shards
     void* bound_user = nullptr;
+    int sampler_map_slots = 3072;               // position-map slots per warp in shared memory (pb200_set_sampler_map_slots)
+    uint64_t sampler_stats[4] = {0, 0, 0, 0};   // last sampler call: users on the shared / global map path, global slots, launches
 };
 
 #define PB_CUDA(ctx, call)                                                              \

@@ -398,6 +398,51 @@ class Engine:
         self._check(st, "gather_dot")
         return out
 
+    def set_sampler_map_slots(self, slots):
+        """shared-memory budget (8-byte slots per warp) of the sampler's position map (pb200_set_sampler_map_slots);
+        users whose map does not fit run with it in global memory.  0 sends every user there."""
+        self._check(self.lib.pb200_set_sampler_map_slots(self.h, int(slots)), "set_sampler_map_slots")
+
+    def sampler_stats(self):
+        """the last sampler call: dict(smem_users, global_users, global_slots, launches) (pb200_sampler_stats)."""
+        out = (C.c_uint64 * 4)()
+        self._check(self.lib.pb200_sampler_stats(self.h, out), "sampler_stats")
+        return dict(smem_users=int(out[0]), global_users=int(out[1]), global_slots=int(out[2]), launches=int(out[3]))
+
+    def _seeds(self, seeds):
+        """uint32 seeds -> device (as the int32 tensor of the same bits)."""
+        if isinstance(seeds, torch.Tensor):
+            return seeds if seeds.dtype == _I32 and seeds.is_cuda else self.upload(seeds.view(torch.int32))
+        return self.upload(np.ascontiguousarray(seeds, dtype=np.uint32).view(np.int32))
+
+    def sample_unseen(self, excl_indptr, excl_indices, seeds, n_items, n_samples, out=None):
+        """the reference's on-the-fly draw of unseen items (pb200_sample_unseen): ``excl_indptr`` int64 / ``excl_indices``
+        int32 CUDA tensors (ordered exclusion lists), ``seeds`` uint32 per user.  Returns int64 [m x n_samples], or fills the
+        first n_samples columns of ``out`` (an int64 CUDA view [m x >= n_samples] with unit column stride)."""
+        m = int(excl_indptr.shape[0]) - 1
+        if out is None:
+            out = self.empty((m, int(n_samples)), torch.int64)
+        sd = self._seeds(seeds)
+        st = self.lib.pb200_sample_unseen(self.h, m, int(n_items), _p(excl_indptr, _I64), _p(excl_indices, _I32), _p(sd, _I32),
+                                          int(n_samples), _p(out, _I64), out.stride(0) if out.dim() > 1 else int(n_samples))
+        self._check(st, "sample_unseen")
+        return out
+
+    def sampled_topk(self, e, v, r, holdout_items, excl_indptr, excl_indices, seeds, n_samples, k, want_scores=False):
+        """sampled evaluation fused (pb200_sampled_topk): top-k positions in ``[holdout | sampled]`` per user.
+        ``holdout_items`` int64 CUDA [m x h]."""
+        m = int(excl_indptr.shape[0]) - 1
+        h = int(holdout_items.shape[1]) if holdout_items.dim() > 1 else 0
+        hold = holdout_items.contiguous()
+        pos = self.empty((m, int(k)), torch.int64)
+        scores = self.empty((m, int(k)), torch.float32) if want_scores else None
+        sd = self._seeds(seeds)
+        st = self.lib.pb200_sampled_topk(self.h, _p(e, _F32), e.stride(0), _p(v, _F32), v.stride(0), m, v.shape[0], int(r),
+                                         _p(hold, _I64), h, _p(excl_indptr, _I64), _p(excl_indices, _I32), _p(sd, _I32),
+                                         int(n_samples), int(k), _p(pos), _p(scores))
+        self._check(st, "sampled_topk")
+        return (pos, scores) if want_scores else pos
+
     def score_dense(self, e, v, r):
         m, n = e.shape[0], v.shape[0]
         s = self.empty((m, n))

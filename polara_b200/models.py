@@ -536,12 +536,21 @@ class _SVDDeviceMixin(_DeviceModelMixin):
         return out.numpy()
 
     # ---- sampled evaluation (RandomSampleEvaluationSVDMixin, models.py:1095-1183) ---------------------------------------
-    def sampled_recommendations(self, holdout_items, unseen_items, test_data=None, shape=None):
+    def sampled_recommendations(self, holdout_items, unseen_items=None, test_data=None, shape=None, n_unseen=None, seed=None,
+                                holdout_users=None):
         """Rank every test user's holdout items against a sample of unseen items (the EIGENREC protocol): scores of the
         ``[n_users x holdout_size]`` holdout items and of the ``[n_users x n_unseen]`` sampled items come from one
         gather-dot over the resident factors (pb200_gather_dot = inner_product_at, lib/sparse.py:58-72), then the top-k
         POSITIONS in the concatenated ``[holdout | unseen]`` row are returned (``np.apply_along_axis(topsort, ...)``,
-        models.py:1182): position < holdout_size means a holdout item was ranked there."""
+        models.py:1182): position < holdout_size means a holdout item was ranked there.
+
+        ``unseen_items=None`` samples them on the fly as the reference does (models.py:1137-1156, 1169-1176): ``n_unseen``
+        items per user, drawn by numba's sampler from the seeds ``SeedSequence(seed).generate_state(n_users)`` and
+        excluding the user's test profile and holdout items, in the order of ``profile + holdout`` as scipy forms it (built
+        on the host, an O(nnz) pass like the reference's; its time is left in ``last_sampled_timings``).  Draw, scoring
+        and ranking are one kernel (pb200_sampled_topk).  ``holdout_users`` (the holdout frame's user column) gives the
+        holdout rows by user runs, as matrix_from_observations does (evaluation.py:45-61); default: ``holdout_size``
+        consecutive entries per user."""
         eng = self.engine
         if test_data is None:
             test_data, shape, _ = self._get_test_data()
@@ -550,6 +559,24 @@ class _SVDDeviceMixin(_DeviceModelMixin):
         v_dev = self._device_factor(f.itemid)
         r_live = self.factors[f.itemid].shape[1]
         e = eng.spmm(p_dev, v_dev, ell=r_live)                       # user_factors = test_matrix.dot(item_factors), :1158
+        if unseen_items is None:
+            if getattr(self, "shard", None) is not None:
+                raise NotImplementedError("on-the-fly sampled evaluation on an item-sharded model")
+            if n_unseen is None:
+                raise ValueError("Number of items to sample is unspecified.")
+            hold = np.asarray(holdout_items, dtype=np.int64)
+            hold = hold.reshape(shape[0], -1)
+            if self.topk > hold.shape[1] + int(n_unseen):
+                raise ValueError("topk exceeds the number of sampled items")
+            t0 = time.perf_counter()
+            indptr, indices = sampled_exclusion_lists(test_data, shape, hold, holdout_users)
+            seeds = np.random.SeedSequence(seed).generate_state(int(shape[0]))
+            t1 = time.perf_counter()
+            pos = eng.sampled_topk(e, v_dev, r_live, eng.upload(hold), eng.upload(indptr), eng.upload(indices), seeds,
+                                   int(n_unseen), self.topk)
+            out = pos.cpu().numpy()
+            self.last_sampled_timings = {"exclusion_ms": (t1 - t0) * 1e3, "device_ms": (time.perf_counter() - t1) * 1e3}
+            return out
         items = np.concatenate([np.asarray(holdout_items, dtype=np.int64).reshape(shape[0], -1),
                                 np.asarray(unseen_items, dtype=np.int64).reshape(shape[0], -1)], axis=1)
         if self.topk > items.shape[1]:
@@ -599,6 +626,33 @@ class _SVDDeviceMixin(_DeviceModelMixin):
         e = eng.spmm(p_dev, v_dev, ell=r_live)
         s = eng.score_dense(e, v_dev, r_live)
         return s.cpu().numpy().astype(np.float64), sl
+
+
+def sampled_exclusion_lists(test_data, shape, holdout_items, holdout_users=None):
+    """Per-user lists of the items the on-the-fly sampler excludes, in the ORDER the reference reads them:
+    ``test_matrix + holdout_matrix`` (models.py:1145-1148) where test_matrix is get_test_matrix's CSR (zero feedback
+    dropped, duplicates summed; models.py:196-211) and holdout_matrix the boolean CSR of matrix_from_observations
+    (evaluation.py:45-61: indices in holdout order, rows = the runs of the holdout users).  scipy adds the two through its
+    general path when a holdout row is unsorted, and the result's order is scipy's -- so scipy forms the sum here too.
+    Returns ``(indptr int64, indices int32)``."""
+    import scipy.sparse as sps_
+    user, item, fdbk = test_data
+    fdbk = np.asarray(fdbk)
+    keep = fdbk != 0
+    n_users, n_items = int(shape[0]), int(shape[1])
+    profile = sps_.csr_matrix((fdbk[keep], (np.asarray(user)[keep], np.asarray(item)[keep])), shape=(n_users, n_items),
+                              dtype=fdbk.dtype)
+    hold = np.asarray(holdout_items).reshape(-1)
+    if holdout_users is None:
+        h = np.asarray(holdout_items).reshape(n_users, -1).shape[1]
+        runs = np.arange(0, len(hold) + 1, max(h, 1), dtype=np.int64) if h else np.zeros(n_users + 1, np.int64)
+    else:
+        keys = np.asarray(holdout_users)
+        runs = np.r_[0, np.where(np.diff(keys))[0] + 1, len(keys)].astype(np.int64)
+    hm = sps_.csr_matrix((n_users, n_items), dtype=bool)
+    hm.data, hm.indices, hm.indptr = np.ones(len(hold), dtype=bool), hold, runs
+    s = profile + hm
+    return s.indptr.astype(np.int64), s.indices.astype(np.int32)
 
 
 def round_tucker_core(core, mode, rank):
@@ -932,8 +986,9 @@ def dropin():
 def dropin_sampled():
     """``PolaraB200SampledSVD``: the device path under the reference's ``RandomSampleEvaluationSVDMixin`` (models.py:1095-
     1183) for data models built with ``RandomSampleEvaluationMixin`` (data.py:938-993) whose unseen interactions were set
-    with ``set_unseen_interactions``.  Sampling on the fly (``unseen_interactions is None``: numba's per-thread Mersenne
-    twister, lib/sampler.py) is not reproduced on the device and raises."""
+    with ``set_unseen_interactions``, or sampled on the fly (``unseen_interactions is None``, ``unseen_items_num`` set):
+    the device draws the same items as numba's sampler (lib/sampler.py) from ``SeedSequence(data.seed)``, models.py:
+    1169-1176.  An item-sharded model raises NotImplementedError there."""
     import pandas as pd
     from polara.recommender.models import RandomSampleEvaluationSVDMixin, SVDModel
 
@@ -946,12 +1001,15 @@ def dropin_sampled():
             userid, itemid = data.fields.userid, data.fields.itemid
             if self._prediction_target == itemid:
                 return _SVDDeviceMixin.get_recommendations(self)
-            if data.unseen_interactions is None:
-                raise NotImplementedError("on-the-fly sampling of unseen items (numba RNG) is not on the device path; "
-                                          "call data.set_unseen_interactions(...) first")
             holdout = data.test.holdout
             assert data.holdout_size >= 1                               # models.py:1106
             holdout_items = holdout[itemid].values.reshape(-1, data.holdout_size)
+            if data.unseen_interactions is None:
+                n_unseen = data.unseen_items_num
+                if n_unseen is None:
+                    raise ValueError('Number of items to sample is unspecified.')     # models.py:1171-1172
+                return self.sampled_recommendations(holdout_items, None, n_unseen=n_unseen, seed=data.seed,
+                                                    holdout_users=holdout[userid].values)
             test_users = holdout[userid].drop_duplicates().values      # preserve sorted (models.py:1123)
             unseen = np.concatenate(data.unseen_interactions.loc[test_users].values).reshape(len(test_users), data.unseen_items_num)
             return self.sampled_recommendations(holdout_items, unseen)
