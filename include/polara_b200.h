@@ -276,6 +276,20 @@ int pb200_sampled_topk(pb200_ctx* ctx, const float* E, int64_t lde, const float*
                        int r, const int64_t* holdout_items, int h, const int64_t* excl_indptr, const int32_t* excl_indices,
                        const uint32_t* seeds_u32, int n_samples, int k, int64_t* out_pos, float* out_scores);
 
+/* pb200_sampled_topk at several truncated ranks of one factor pair in one pass: the rank sweep of find_optimal_svd_rank
+ * (evaluation/pipelines.py:81-116, truncation models.py:819-832) under the sampled protocol.  Each user is drawn once;
+ * each drawn (and holdout) item's fp32 chain is continued from ranks[j-1] to ranks[j] and offered to list j, so each V
+ * row is read once, up to the largest rank.  ranks_host: host array of n_ranks ints, strictly ascending,
+ * 1 <= ranks[0], ranks[n_ranks-1] <= min(lde, ldv), 1 <= n_ranks <= 64.  out_pos int64 [n_ranks x m x k], rank-major
+ * (block j has the layout of pb200_sampled_topk's output), out_scores float32 of the same layout or NULL.  For every j,
+ * block j is bit-equal to pb200_sampled_topk(E, lde, V, ldv, m, n, ranks[j], ...) on the same E and V.  Errors and
+ * synchronisation as pb200_sampled_topk, plus PB200_EINVAL for a rank list that is empty, too long, not strictly
+ * ascending, below 1 or above lde / ldv. */
+int pb200_sampled_topk_ranks(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int64_t ldv, int64_t m, int64_t n,
+                             const int* ranks_host, int n_ranks, const int64_t* holdout_items, int h,
+                             const int64_t* excl_indptr, const int32_t* excl_indices, const uint32_t* seeds_u32,
+                             int n_samples, int k, int64_t* out_pos, float* out_scores);
+
 /* Position-map placement of the two sampler entries: a user whose map (2 * |exclusion| + n_samples entries at most, at a
  * load factor <= 2/3) fits in `slots` 8-byte slots runs with the map in shared memory, the others with it in global
  * memory.  0..6144, default 3072; 0 puts every user on the global-memory path.  Results do not depend on it. */

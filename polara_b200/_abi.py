@@ -64,6 +64,8 @@ _SIGNATURES = {
     "pb200_sample_unseen": ([ptr, i64, i64, ptr, ptr, ptr, C.c_int, ptr, i64], C.c_int),
     "pb200_sampled_topk": ([ptr, ptr, i64, ptr, i64, i64, i64, C.c_int, ptr, C.c_int, ptr, ptr, ptr, C.c_int, C.c_int, ptr,
                             ptr], C.c_int),
+    "pb200_sampled_topk_ranks": ([ptr, ptr, i64, ptr, i64, i64, i64, ptr, C.c_int, ptr, C.c_int, ptr, ptr, ptr, C.c_int,
+                                  C.c_int, ptr, ptr], C.c_int),
     "pb200_set_sampler_map_slots": ([ptr, C.c_int], C.c_int),
     "pb200_sampler_stats": ([ptr, C.POINTER(C.c_uint64)], C.c_int),
     "pb200_score_dense": ([ptr, ptr, i64, ptr, i64, i64, i64, C.c_int, ptr, i64], C.c_int),

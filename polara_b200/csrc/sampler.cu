@@ -2,7 +2,9 @@
 // polara/recommender/models.py:1137-1183), reproducing the reference's draws bit for bit:
 //   pb200_sample_unseen   sample_row_wise (polara/lib/sampler.py:96-111): the item ids only;
 //   pb200_sampled_topk    mf_random_item_scoring (sampler.py:73-93) + the concatenation with the holdout scores and the
-//                         per-row topsort (models.py:1178-1183), fused: no [m x (h + n_samples)] block reaches HBM.
+//                         per-row topsort (models.py:1178-1183), fused: no [m x (h + n_samples)] block reaches HBM;
+//   pb200_sampled_topk_ranks  the same at several truncated ranks of one factor pair (find_optimal_svd_rank,
+//                         evaluation/pipelines.py:81-116): one draw per user, one score chain per item, one list per rank.
 //
 // The reference, per user: numba's random.seed(seed) (MT19937 init_genrand), prime_sampler_state (excluded items moved
 // to the tail of range(n) in LIST order through two dicts, `state` position -> item and `track` item -> position), then
@@ -29,6 +31,8 @@ constexpr unsigned long long EMPTY = ~0ull;
 constexpr uint32_t TRACK = 0x80000000u;                  // tag of `track` keys (ids are < 2^31)
 constexpr int MAX_SMEM_SLOTS = 6144;                      // 4 warps x (2.5 KB MT + 48 KB map) fits one block per SM
 constexpr size_t GLOBAL_MAP_BUDGET = size_t(256) << 20;  // bytes of global tables in flight
+constexpr size_t GLOBAL_LIST_BUDGET = size_t(256) << 20; // bytes of running lists of the global-path warps
+constexpr int MAX_RANKS = 64;                             // ranks per fused call (kept in the kernel parameters)
 
 // table size for a user: the entry bound 2L + s at a load factor <= 2/3, plus a floor
 __host__ __device__ __forceinline__ int64_t map_slots_for(int64_t L, int64_t s) {
@@ -136,12 +140,13 @@ struct Params {
     int64_t lde;
     const float* V;
     int64_t ldv;
-    int r;
+    int nr;                                                // truncated ranks, strictly ascending
+    int ranks[MAX_RANKS];
     const int64_t* holdout;                                // [m x h]
     int h, k;
-    int64_t* out_pos;
+    int64_t* out_pos;                                      // [nr x m x k], rank-major
     float* out_scores;
-    pb200_cand* lists;                                     // [warps in the grid x k] running top-k lists
+    pb200_cand* lists;                                     // [warps in the grid x nr x k] running top-k lists
     // map placement
     int smem_slots;                                        // shared-memory path: slots per warp
     const int64_t* heavy;                                  // global path: users, count, table slots per warp
@@ -163,8 +168,44 @@ __device__ __forceinline__ void offer(pb200_cand* list, int k, int& cnt, float& 
     }
 }
 
+// exact_score's chain continued over columns [t0, t1)
+__device__ __forceinline__ float score_chain(const float* __restrict__ e, const float* __restrict__ v, int t0, int t1,
+                                             float s) {
+    for (int t = t0; t < t1; ++t) s = fmaf(e[t], v[t], s);
+    return s;
+}
+
+// One batch of up to 32 items, lane t holding item `item` (valid if `have`) at row position `pos`, offered to the list
+// of every rank: the lane's score chain fmaf(e[t], v[t], s), t ascending from 0, is continued from ranks[j-1] to
+// ranks[j] before list j sees it, so list j gets exactly exact_score(e, v, ranks[j]) and each V row is read once.  Ids
+// out of [0, n) score NaN at every rank and never enter.  List 0's fill and threshold are plain registers (cnt0 / thr0:
+// the single-rank call keeps the code it had; read back through a shuffle, they are no longer known to be warp-uniform
+// and the list insertions run ~5 % slower); list j >= 1's live in lane j % 32 of cnt_lo/thr_lo (j < 32) or
+// cnt_hi/thr_hi, out of local memory.
+__device__ __forceinline__ void offer_ranks(const Params& p, const float* e, pb200_cand* lists, int& cnt0, float& thr0,
+                                            int& cnt_lo, int& cnt_hi, float& thr_lo, float& thr_hi, bool have, int64_t item,
+                                            int pos, int lane) {
+    const bool valid = have && item >= 0 && item < p.n;
+    const float* v = p.V + (valid ? item : 0) * p.ldv;
+    int t = p.ranks[0];
+    float s = valid ? score_chain(e, v, 0, t, 0.f) : 0.f;
+    offer(lists, p.k, cnt0, thr0, have, valid ? s : CUDART_NAN_F, pos, lane);
+    for (int j = 1; j < p.nr; ++j) {
+        const int rj = p.ranks[j];
+        if (valid) s = score_chain(e, v, t, rj, s);
+        t = rj;
+        const bool hi = j >= 32;
+        int cnt = __shfl_sync(0xffffffffu, hi ? cnt_hi : cnt_lo, j & 31);
+        float thr = __shfl_sync(0xffffffffu, hi ? thr_hi : thr_lo, j & 31);
+        offer(lists + (int64_t)j * p.k, p.k, cnt, thr, have, valid ? s : CUDART_NAN_F, pos, lane);
+        if (lane == (j & 31)) {
+            if (hi) { cnt_hi = cnt; thr_hi = thr; } else { cnt_lo = cnt; thr_lo = thr; }
+        }
+    }
+}
+
 template <bool FUSED>
-__device__ void run_user(const Params& p, int64_t u, uint32_t* mt, Map map, pb200_cand* list, int lane) {
+__device__ void run_user(const Params& p, int64_t u, uint32_t* mt, Map map, pb200_cand* lists, int lane) {
     const int64_t b = p.excl_indptr[u], L = p.excl_indptr[u + 1] - b;
     // random.seed(seeds[u]): init_genrand
     if (lane == 0) {
@@ -196,20 +237,16 @@ __device__ void run_user(const Params& p, int64_t u, uint32_t* mt, Map map, pb20
         }
     }
     __syncwarp();
-    int cnt = 0;
-    float thr = -CUDART_INF_F;
+    int cnt0 = 0, cnt_lo = 0, cnt_hi = 0;
+    float thr0 = -CUDART_INF_F, thr_lo = -CUDART_INF_F, thr_hi = -CUDART_INF_F;
     const float* e = nullptr;
     if (FUSED) {
         e = p.E + u * p.lde;
         // holdout items first: positions 0 .. h-1 (pb200_gather_dot's scores: NaN for ids out of range)
         for (int c0 = 0; c0 < p.h; c0 += 32) {
             const int j = c0 + lane;
-            float x = CUDART_NAN_F;
-            if (j < p.h) {
-                const int64_t it = p.holdout[u * p.h + j];
-                if (it >= 0 && it < p.n) x = exact_score(e, p.V + it * p.ldv, p.r);
-            }
-            offer(list, p.k, cnt, thr, j < p.h, x, j, lane);
+            const int64_t it = j < p.h ? p.holdout[u * p.h + j] : -1;
+            offer_ranks(p, e, lists, cnt0, thr0, cnt_lo, cnt_hi, thr_lo, thr_hi, j < p.h, it, j, lane);
         }
     }
     // sample_fill
@@ -231,18 +268,22 @@ __device__ void run_user(const Params& p, int64_t u, uint32_t* mt, Map map, pb20
             if (lane == (j & 31)) held = item;
             if ((j & 31) == 31 || j == p.s - 1) {
                 const int c0 = j & ~31;
-                const bool have = c0 + lane <= j;
-                const float x = have ? exact_score(e, p.V + (int64_t)held * p.ldv, p.r) : 0.f;
-                offer(list, p.k, cnt, thr, have, x, p.h + c0 + lane, lane);
+                offer_ranks(p, e, lists, cnt0, thr0, cnt_lo, cnt_hi, thr_lo, thr_hi, c0 + lane <= j, (int64_t)held,
+                            p.h + c0 + lane, lane);
             }
         }
     }
     if (FUSED) {
         __syncwarp();
-        for (int i = lane; i < p.k; i += 32) {
-            const bool ok = i < cnt;
-            p.out_pos[u * p.k + i] = ok ? (int64_t)list[i].id : -1;
-            if (p.out_scores) p.out_scores[u * p.k + i] = ok ? list[i].score : -CUDART_INF_F;
+        for (int j = 0; j < p.nr; ++j) {
+            const int cnt = j == 0 ? cnt0 : __shfl_sync(0xffffffffu, j >= 32 ? cnt_hi : cnt_lo, j & 31);
+            const pb200_cand* list = lists + (int64_t)j * p.k;
+            const int64_t o = ((int64_t)j * p.m + u) * p.k;
+            for (int i = lane; i < p.k; i += 32) {
+                const bool ok = i < cnt;
+                p.out_pos[o + i] = ok ? (int64_t)list[i].id : -1;
+                if (p.out_scores) p.out_scores[o + i] = ok ? list[i].score : -CUDART_INF_F;
+            }
         }
         __syncwarp();
     }
@@ -257,27 +298,29 @@ __global__ void __launch_bounds__(WARPS * 32) sampler_smem_kernel(Params p) {
     uint32_t* mt = reinterpret_cast<uint32_t*>(smem + w * per_warp);
     unsigned long long* slots = reinterpret_cast<unsigned long long*>(mt + MT_N);
     const int64_t gw = (int64_t)blockIdx.x * WARPS + w, nw = (int64_t)gridDim.x * WARPS;
-    pb200_cand* list = FUSED ? p.lists + gw * p.k : nullptr;
+    pb200_cand* lists = FUSED ? p.lists + gw * p.nr * p.k : nullptr;
     for (int64_t u = gw; u < p.m; u += nw) {
         const int64_t L = p.excl_indptr[u + 1] - p.excl_indptr[u];
         const int64_t cap = map_slots_for(L, p.s);
         if (cap > p.smem_slots) continue;
-        run_user<FUSED>(p, u, mt, Map{slots, (uint32_t)cap}, list, lane);
+        run_user<FUSED>(p, u, mt, Map{slots, (uint32_t)cap}, lists, lane);
     }
 }
 
-// users whose table does not fit: one table of p.gslots slots per warp in global memory
+// users whose table does not fit: one table of p.gslots slots per warp in global memory.  The minimum block counts hold
+// each variant at the register count it needs without spilling (left alone, ptxas caps the fused one at 56 and spills;
+// it needs 80)
 template <bool FUSED>
-__global__ void __launch_bounds__(WARPS * 32) sampler_gmem_kernel(Params p) {
+__global__ void __launch_bounds__(WARPS * 32, FUSED ? 6 : 10) sampler_gmem_kernel(Params p) {
     __shared__ uint32_t mts[WARPS][MT_N];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const int64_t gw = (int64_t)blockIdx.x * WARPS + w, nw = (int64_t)gridDim.x * WARPS;
-    pb200_cand* list = FUSED ? p.lists + gw * p.k : nullptr;
+    pb200_cand* lists = FUSED ? p.lists + gw * p.nr * p.k : nullptr;
     unsigned long long* slots = p.gmaps + gw * p.gslots;
     for (int64_t t = gw; t < p.n_heavy; t += nw) {
         const int64_t u = p.heavy[t];
         const int64_t L = p.excl_indptr[u + 1] - p.excl_indptr[u];
-        run_user<FUSED>(p, u, mts[w], Map{slots, (uint32_t)map_slots_for(L, p.s)}, list, lane);
+        run_user<FUSED>(p, u, mts[w], Map{slots, (uint32_t)map_slots_for(L, p.s)}, lists, lane);
     }
 }
 
@@ -352,7 +395,7 @@ int sampler_run(pb200_ctx* ctx, Params p, bool fused) {
         PB_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&dev_max_blocks, kern, WARPS * 32, smem));
         const int64_t blocks = std::max<int64_t>(1, std::min<int64_t>(ceil_div64(p.m, WARPS),
                                                                       (int64_t)std::max(dev_max_blocks, 1) * ctx->num_sms));
-        if (fused) PB_TRY(sc.alloc(&p.lists, (size_t)blocks * WARPS * p.k));
+        if (fused) PB_TRY(sc.alloc(&p.lists, (size_t)blocks * WARPS * p.nr * p.k));
         kern<<<(unsigned)blocks, WARPS * 32, smem, ctx->stream>>>(p);
         PB_CUDA(ctx, cudaGetLastError());
         ctx->stats[0] += 1;
@@ -362,13 +405,16 @@ int sampler_run(pb200_ctx* ctx, Params p, bool fused) {
         const int64_t gslots = (int64_t)hf[3];
         PB_REQUIRE(ctx, gslots < (int64_t)UINT32_MAX, "sample_unseen: exclusion list too long");
         const int64_t by_mem = std::max<int64_t>(1, (int64_t)(GLOBAL_MAP_BUDGET / ((size_t)gslots * 8)));
-        const int64_t warps = std::min<int64_t>({n_heavy, by_mem, (int64_t)ctx->num_sms * 16 * WARPS});
+        const int64_t by_lists = fused ? std::max<int64_t>(1, (int64_t)(GLOBAL_LIST_BUDGET / ((size_t)p.nr * p.k *
+                                                                                                sizeof(pb200_cand))))
+                                       : n_heavy;
+        const int64_t warps = std::min<int64_t>({n_heavy, by_mem, by_lists, (int64_t)ctx->num_sms * 16 * WARPS});
         const int64_t blocks = ceil_div64(warps, WARPS);
         p.heavy = heavy;
         p.n_heavy = n_heavy;
         p.gslots = gslots;
         PB_TRY(sc.alloc(&p.gmaps, (size_t)blocks * WARPS * gslots));
-        if (fused) PB_TRY(sc.alloc(&p.lists, (size_t)blocks * WARPS * p.k));
+        if (fused) PB_TRY(sc.alloc(&p.lists, (size_t)blocks * WARPS * p.nr * p.k));
         auto kern = fused ? sampler_gmem_kernel<true> : sampler_gmem_kernel<false>;
         kern<<<(unsigned)blocks, WARPS * 32, 0, ctx->stream>>>(p);
         PB_CUDA(ctx, cudaGetLastError());
@@ -408,20 +454,51 @@ extern "C" int pb200_sample_unseen(pb200_ctx* ctx, int64_t m, int64_t n_items, c
     return sampler_run(ctx, p, false);
 }
 
+// pb200_sampled_topk / pb200_sampled_topk_ranks: one routine; the single-rank entry is the rank list {r}
+static int sampled_topk_run(pb200_ctx* ctx, const char* where, const float* E, int64_t lde, const float* V, int64_t ldv,
+                     int64_t m, int64_t n, const int* ranks, int n_ranks, const int64_t* holdout_items, int h,
+                     const int64_t* excl_indptr, const int32_t* excl_indices, const uint32_t* seeds_u32, int n_samples,
+                     int k, int64_t* out_pos, float* out_scores) {
+    const std::string w(where);
+    PB_REQUIRE(ctx, m >= 0 && n > 0 && n < (int64_t)2147483647 && lde > 0 && ldv > 0, (w + ": bad shape").c_str());
+    PB_REQUIRE(ctx, h >= 0 && n_samples >= 0, (w + ": negative holdout or sample size").c_str());
+    PB_REQUIRE(ctx, k >= 1 && (int64_t)k <= (int64_t)h + n_samples, (w + ": k must be in 1..h + n_samples").c_str());
+    Params p{};
+    p.nr = n_ranks;
+    for (int j = 0; j < n_ranks; ++j) p.ranks[j] = ranks[j];
+    if (m == 0) return PB200_OK;
+    PB_REQUIRE(ctx, E && V && (holdout_items || h == 0) && excl_indptr && excl_indices && seeds_u32 && out_pos,
+               (w + ": null argument").c_str());
+    p.m = m; p.n = n; p.excl_indptr = excl_indptr; p.excl_indices = excl_indices; p.seeds = seeds_u32; p.s = n_samples;
+    p.E = E; p.lde = lde; p.V = V; p.ldv = ldv; p.holdout = holdout_items; p.h = h; p.k = k;
+    p.out_pos = out_pos; p.out_scores = out_scores;
+    return sampler_run(ctx, p, true);
+}
+
 extern "C" int pb200_sampled_topk(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int64_t ldv, int64_t m,
                                   int64_t n, int r, const int64_t* holdout_items, int h, const int64_t* excl_indptr,
                                   const int32_t* excl_indices, const uint32_t* seeds_u32, int n_samples, int k,
                                   int64_t* out_pos, float* out_scores) {
     PB_ENTER(ctx);
-    PB_REQUIRE(ctx, m >= 0 && n > 0 && n < (int64_t)2147483647 && r > 0 && lde >= r && ldv >= r, "sampled_topk: bad shape");
-    PB_REQUIRE(ctx, h >= 0 && n_samples >= 0, "sampled_topk: negative holdout or sample size");
-    PB_REQUIRE(ctx, k >= 1 && (int64_t)k <= (int64_t)h + n_samples, "sampled_topk: k must be in 1..h + n_samples");
-    if (m == 0) return PB200_OK;
-    PB_REQUIRE(ctx, E && V && (holdout_items || h == 0) && excl_indptr && excl_indices && seeds_u32 && out_pos,
-               "sampled_topk: null argument");
-    Params p{};
-    p.m = m; p.n = n; p.excl_indptr = excl_indptr; p.excl_indices = excl_indices; p.seeds = seeds_u32; p.s = n_samples;
-    p.E = E; p.lde = lde; p.V = V; p.ldv = ldv; p.r = r; p.holdout = holdout_items; p.h = h; p.k = k;
-    p.out_pos = out_pos; p.out_scores = out_scores;
-    return sampler_run(ctx, p, true);
+    PB_REQUIRE(ctx, r > 0 && lde >= r && ldv >= r, "sampled_topk: bad shape");
+    return sampled_topk_run(ctx, "sampled_topk", E, lde, V, ldv, m, n, &r, 1, holdout_items, h, excl_indptr,
+                            excl_indices, seeds_u32, n_samples, k, out_pos, out_scores);
+}
+
+extern "C" int pb200_sampled_topk_ranks(pb200_ctx* ctx, const float* E, int64_t lde, const float* V, int64_t ldv,
+                                        int64_t m, int64_t n, const int* ranks_host, int n_ranks,
+                                        const int64_t* holdout_items, int h, const int64_t* excl_indptr,
+                                        const int32_t* excl_indices, const uint32_t* seeds_u32, int n_samples, int k,
+                                        int64_t* out_pos, float* out_scores) {
+    PB_ENTER(ctx);
+    PB_REQUIRE(ctx, ranks_host && n_ranks >= 1 && n_ranks <= MAX_RANKS,
+               "sampled_topk_ranks: the rank list must hold 1..64 ranks");
+    for (int j = 0; j < n_ranks; ++j) {
+        PB_REQUIRE(ctx, ranks_host[j] >= 1, "sampled_topk_ranks: ranks must be >= 1");
+        PB_REQUIRE(ctx, j == 0 || ranks_host[j] > ranks_host[j - 1], "sampled_topk_ranks: ranks must be strictly ascending");
+    }
+    PB_REQUIRE(ctx, (int64_t)ranks_host[n_ranks - 1] <= lde && (int64_t)ranks_host[n_ranks - 1] <= ldv,
+               "sampled_topk_ranks: the largest rank exceeds lde or ldv");
+    return sampled_topk_run(ctx, "sampled_topk_ranks", E, lde, V, ldv, m, n, ranks_host, n_ranks, holdout_items, h,
+                            excl_indptr, excl_indices, seeds_u32, n_samples, k, out_pos, out_scores);
 }

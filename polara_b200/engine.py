@@ -433,7 +433,7 @@ class Engine:
         ``holdout_items`` int64 CUDA [m x h]."""
         m = int(excl_indptr.shape[0]) - 1
         h = int(holdout_items.shape[1]) if holdout_items.dim() > 1 else 0
-        hold = holdout_items.contiguous()
+        hold = holdout_items.contiguous() if h else None          # an [m x 0] tensor has no usable strides
         pos = self.empty((m, int(k)), torch.int64)
         scores = self.empty((m, int(k)), torch.float32) if want_scores else None
         sd = self._seeds(seeds)
@@ -441,6 +441,26 @@ class Engine:
                                          _p(hold, _I64), h, _p(excl_indptr, _I64), _p(excl_indices, _I32), _p(sd, _I32),
                                          int(n_samples), int(k), _p(pos), _p(scores))
         self._check(st, "sampled_topk")
+        return (pos, scores) if want_scores else pos
+
+    def sampled_topk_ranks(self, e, v, ranks, holdout_items, excl_indptr, excl_indices, seeds, n_samples, k,
+                           want_scores=False):
+        """``sampled_topk`` at every rank of ``ranks`` (strictly ascending) with one draw per user
+        (pb200_sampled_topk_ranks): returns positions int64 ``[R, m, k]``, block j bit-equal to
+        ``sampled_topk(e, v, ranks[j], ...)``."""
+        m = int(excl_indptr.shape[0]) - 1
+        h = int(holdout_items.shape[1]) if holdout_items.dim() > 1 else 0
+        hold = holdout_items.contiguous() if h else None          # an [m x 0] tensor has no usable strides
+        ranks = [int(r) for r in ranks]
+        rk = (C.c_int * max(len(ranks), 1))(*ranks)
+        pos = self.empty((len(ranks), m, int(k)), torch.int64)
+        scores = self.empty((len(ranks), m, int(k)), torch.float32) if want_scores else None
+        sd = self._seeds(seeds)
+        st = self.lib.pb200_sampled_topk_ranks(self.h, _p(e, _F32), e.stride(0), _p(v, _F32), v.stride(0), m, v.shape[0],
+                                               C.cast(rk, C.c_void_p), len(ranks), _p(hold, _I64), h, _p(excl_indptr, _I64),
+                                               _p(excl_indices, _I32), _p(sd, _I32), int(n_samples), int(k), _p(pos),
+                                               _p(scores))
+        self._check(st, "sampled_topk_ranks")
         return (pos, scores) if want_scores else pos
 
     def score_dense(self, e, v, r):

@@ -403,7 +403,7 @@ class RecommenderModel:
         f = self.data.fields
         holdout = self.data.test.holdout
         h_user = np.asarray(holdout[f.userid].values, dtype=np.int64)
-        h_item = np.asarray(holdout[f.itemid].values, dtype=np.int64)
+        h_item = np.asarray(holdout[self._prediction_target].values, dtype=np.int64)     # assemble_scoring_matrices
         h_fdbk = None if (f.feedback is None or ignore_feedback) else np.asarray(holdout[f.feedback].values)
         if f.feedback is None:
             switch_positive = None

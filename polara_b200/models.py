@@ -548,20 +548,77 @@ class _SVDDeviceMixin(_DeviceModelMixin):
         items per user, drawn by numba's sampler from the seeds ``SeedSequence(seed).generate_state(n_users)`` and
         excluding the user's test profile and holdout items, in the order of ``profile + holdout`` as scipy forms it (built
         on the host, an O(nnz) pass like the reference's; its time is left in ``last_sampled_timings``).  Draw, scoring
-        and ranking are one kernel (pb200_sampled_topk).  ``holdout_users`` (the holdout frame's user column) gives the
+        and ranking are one kernel (the routine of pb200_sampled_topk, called through pb200_sampled_topk_ranks with the
+        one live rank).  ``holdout_users`` (the holdout frame's user column) gives the
         holdout rows by user runs, as matrix_from_observations does (evaluation.py:45-61); default: ``holdout_size``
         consecutive entries per user."""
+        if unseen_items is None and getattr(self, "shard", None) is not None:
+            raise NotImplementedError("on-the-fly sampled evaluation on an item-sharded model")
+        r_live = self.factors[self.data.fields.itemid].shape[1]
+        return self._sampled_lists([r_live], holdout_items, unseen_items, test_data, shape, n_unseen, seed,
+                                   holdout_users)[0]
+
+    def sampled_rank_sweep(self, ranks, holdout_items, unseen_items=None, n_unseen=None, seed=None, holdout_users=None,
+                           test_data=None, shape=None):
+        """``sampled_recommendations`` at every rank of ``ranks`` on the current factors truncated to that rank (the loop
+        of find_optimal_svd_rank, evaluation/pipelines.py:81-116, with the truncation of models.py:819-832), made once:
+        one exclusion-list pass, one SpMM at the largest rank and, drawn on the fly, one kernel that draws each user's
+        items once and ranks them at every rank (pb200_sampled_topk_ranks).  With pre-sampled ``unseen_items`` there is
+        no draw to share: one gather-dot + top-k per rank on the leading columns of the same embeddings.  Arguments as
+        ``sampled_recommendations``.  Returns ``{rank: positions}``.
+
+        The embeddings are the leading columns of ``P V`` at the largest rank, as the reference takes them; in fp32 a
+        column's sum order depends on the SpMM kernel its column group runs on, so the lists can differ from those of a
+        model truncated to that rank in the last bits of near-tied scores (DESIGN.md section 4)."""
+        ranks = self._sweep_ranks(ranks)
+        lists = self._sampled_lists(ranks, holdout_items, unseen_items, test_data, shape, n_unseen, seed, holdout_users)
+        return dict(zip(ranks, lists))
+
+    def rank_sweep(self, ranks):
+        """``get_recommendations`` (standard protocol) at every rank of ``ranks`` on the current factors truncated to that
+        rank, made once: one test-data ingest, one SpMM at the largest rank (through the right item projector for a model
+        that carries HybridSVD projectors), then the fused scoring kernel once per rank on the leading columns of the
+        same embeddings, honouring ``filter_seen`` and ``score_kernel``.  Returns ``{rank: int64 [n_test_users x topk]}``.
+        The test triplets are read as ``get_recommendations`` reads them (``_big_test_triplets`` for large test sets,
+        else ``_get_test_data``).  Same note on the embeddings as ``sampled_rank_sweep``."""
+        ranks = self._sweep_ranks(ranks)
+        if self.verify_integrity and hasattr(self, "verify_data_integrity"):
+            self.verify_data_integrity()
+        eng = self.engine
+        big = self._big_test_triplets()
+        test_data, shape = big if big is not None else self._get_test_data()[:2]
+        if self.topk > shape[1]:
+            raise ValueError("topk exceeds the number of items")
+        p_dev, seen_dev = self._test_csr_device(test_data, shape, sorted_users=big is not None)
+        v_dev = self._device_factor(self.data.fields.itemid)
+        if self.score_kernel is not None:
+            eng.set_score_kernel(self.score_kernel)
+        v_fold, v_score = self._item_projector_device(v_dev)
+        e = eng.spmm(p_dev, v_fold, ell=min(v_fold.shape[1], round_up(ranks[-1], 32)))
+        seen = seen_dev if self.filter_seen else None
+        return {r: eng.score_topk(e, v_score, r, self.topk, seen=seen).cpu().numpy() for r in ranks}
+
+    def _sweep_ranks(self, ranks):
+        """the distinct ranks of a sweep, ascending; each must be a truncation of the current factors."""
+        if getattr(self, "shard", None) is not None:
+            raise NotImplementedError("rank sweep on an item-sharded model")
+        ranks = sorted({int(r) for r in ranks})
+        width = self.factors[self.data.fields.itemid].shape[1]
+        if not ranks or ranks[0] < 1 or ranks[-1] > width:
+            raise ValueError("sweep ranks must be in 1..%d, the width of the current factors (a larger rank needs a "
+                             "rebuild); got %s" % (width, ranks))
+        return ranks
+
+    def _sampled_lists(self, ranks, holdout_items, unseen_items, test_data, shape, n_unseen, seed, holdout_users):
+        """the sampled protocol's top-k positions at each of the ascending ``ranks``, as a list."""
         eng = self.engine
         if test_data is None:
             test_data, shape, _ = self._get_test_data()
         f = self.data.fields
         p_dev, _ = self._test_csr_device(test_data, shape)
         v_dev = self._device_factor(f.itemid)
-        r_live = self.factors[f.itemid].shape[1]
-        e = eng.spmm(p_dev, v_dev, ell=r_live)                       # user_factors = test_matrix.dot(item_factors), :1158
+        e = eng.spmm(p_dev, v_dev, ell=ranks[-1])                    # user_factors = test_matrix.dot(item_factors), :1158
         if unseen_items is None:
-            if getattr(self, "shard", None) is not None:
-                raise NotImplementedError("on-the-fly sampled evaluation on an item-sharded model")
             if n_unseen is None:
                 raise ValueError("Number of items to sample is unspecified.")
             hold = np.asarray(holdout_items, dtype=np.int64)
@@ -572,9 +629,9 @@ class _SVDDeviceMixin(_DeviceModelMixin):
             indptr, indices = sampled_exclusion_lists(test_data, shape, hold, holdout_users)
             seeds = np.random.SeedSequence(seed).generate_state(int(shape[0]))
             t1 = time.perf_counter()
-            pos = eng.sampled_topk(e, v_dev, r_live, eng.upload(hold), eng.upload(indptr), eng.upload(indices), seeds,
-                                   int(n_unseen), self.topk)
-            out = pos.cpu().numpy()
+            pos = eng.sampled_topk_ranks(e, v_dev, ranks, eng.upload(hold), eng.upload(indptr), eng.upload(indices), seeds,
+                                         int(n_unseen), self.topk)
+            out = list(pos.cpu().numpy())
             self.last_sampled_timings = {"exclusion_ms": (t1 - t0) * 1e3, "device_ms": (time.perf_counter() - t1) * 1e3}
             return out
         items = np.concatenate([np.asarray(holdout_items, dtype=np.int64).reshape(shape[0], -1),
@@ -582,8 +639,8 @@ class _SVDDeviceMixin(_DeviceModelMixin):
         if self.topk > items.shape[1]:
             raise ValueError("topk exceeds the number of sampled items")
         users = np.broadcast_to(np.arange(shape[0], dtype=np.int64)[:, None], items.shape)
-        scores = eng.gather_dot(e, v_dev, r_live, eng.upload(np.ascontiguousarray(users)), eng.upload(items))
-        return eng.topk_dense(scores, self.topk).cpu().numpy()
+        u_dev, i_dev = eng.upload(np.ascontiguousarray(users)), eng.upload(items)
+        return [eng.topk_dense(eng.gather_dot(e, v_dev, r, u_dev, i_dev), self.topk).cpu().numpy() for r in ranks]
 
     # ---- item cold start (ItemColdStartSVDModelMixin.slice_recommendations, coldstart/models.py:216-222) ---------------
     def coldstart_recommendations(self, cold_item_features, feature_embeddings, transform_helper):
@@ -653,6 +710,26 @@ def sampled_exclusion_lists(test_data, shape, holdout_items, holdout_users=None)
     hm.data, hm.indices, hm.indptr = np.ones(len(hold), dtype=bool), hold, runs
     s = profile + hm
     return s.indptr.astype(np.int64), s.indices.astype(np.int32)
+
+
+def sampled_protocol_inputs(model):
+    """What the sampled protocol reads from a ``RandomSampleEvaluationMixin`` data model (data.py:938-993,
+    models.py:1095-1183): ``(holdout_items [n_users x holdout_size], unseen_items, kwargs)`` -- ``unseen_items`` the
+    pre-sampled items of ``set_unseen_interactions`` with empty ``kwargs``, or None with the on-the-fly draw's
+    ``n_unseen`` / ``seed`` / ``holdout_users``."""
+    data = model.data
+    userid, itemid = data.fields.userid, data.fields.itemid
+    holdout = data.test.holdout
+    assert data.holdout_size >= 1                               # models.py:1106
+    holdout_items = holdout[itemid].values.reshape(-1, data.holdout_size)
+    if data.unseen_interactions is None:
+        if data.unseen_items_num is None:
+            raise ValueError('Number of items to sample is unspecified.')     # models.py:1171-1172
+        return holdout_items, None, dict(n_unseen=data.unseen_items_num, seed=data.seed,
+                                         holdout_users=holdout[userid].values)
+    test_users = holdout[userid].drop_duplicates().values      # preserve sorted (models.py:1123)
+    unseen = np.concatenate(data.unseen_interactions.loc[test_users].values).reshape(len(test_users), data.unseen_items_num)
+    return holdout_items, unseen, {}
 
 
 def round_tucker_core(core, mode, rank):
@@ -997,21 +1074,17 @@ def dropin_sampled():
             return _SVDDeviceMixin.build(self, operator=operator, return_factors=return_factors)
 
         def get_recommendations(self):
-            data = self.data
-            userid, itemid = data.fields.userid, data.fields.itemid
-            if self._prediction_target == itemid:
+            if self._prediction_target == self.data.fields.itemid:
                 return _SVDDeviceMixin.get_recommendations(self)
-            holdout = data.test.holdout
-            assert data.holdout_size >= 1                               # models.py:1106
-            holdout_items = holdout[itemid].values.reshape(-1, data.holdout_size)
-            if data.unseen_interactions is None:
-                n_unseen = data.unseen_items_num
-                if n_unseen is None:
-                    raise ValueError('Number of items to sample is unspecified.')     # models.py:1171-1172
-                return self.sampled_recommendations(holdout_items, None, n_unseen=n_unseen, seed=data.seed,
-                                                    holdout_users=holdout[userid].values)
-            test_users = holdout[userid].drop_duplicates().values      # preserve sorted (models.py:1123)
-            unseen = np.concatenate(data.unseen_interactions.loc[test_users].values).reshape(len(test_users), data.unseen_items_num)
-            return self.sampled_recommendations(holdout_items, unseen)
+            holdout_items, unseen, kwargs = sampled_protocol_inputs(self)
+            return self.sampled_recommendations(holdout_items, unseen, **kwargs)
+
+        def rank_sweep(self, ranks):
+            """the lists of ``get_recommendations`` at every rank of ``ranks`` (``{rank: lists}``), dispatched on
+            ``_prediction_target`` as ``get_recommendations`` is: the standard sweep for items, else the sampled one."""
+            if self._prediction_target == self.data.fields.itemid:
+                return _SVDDeviceMixin.rank_sweep(self, ranks)
+            holdout_items, unseen, kwargs = sampled_protocol_inputs(self)
+            return self.sampled_rank_sweep(ranks, holdout_items, unseen, **kwargs)
 
     return PolaraB200SampledSVD

@@ -1,0 +1,93 @@
+"""Rank search of an SVD model with the lists of every rank computed in one device sweep.
+
+:func:`find_optimal_svd_rank` has the signature and the semantics of ``polara.evaluation.pipelines.find_optimal_svd_rank``
+(pipelines.py:81-116): build once at the largest rank, then evaluate the truncated model at each rank, largest first.
+The reference recomputes the recommendations at every rank; here they come from one call made before the loop --
+``rank_sweep`` for the standard protocol, ``sampled_rank_sweep`` for sampled evaluation -- which shares the test-data
+ingest, the SpMM at the largest rank and, on the sampled protocol, the draw of the unseen items between all ranks.  The
+evaluator then sees the model at each rank with ``_recommendations`` set to that rank's lists.
+"""
+from __future__ import annotations
+
+from collections.abc import Iterable, Mapping
+
+from .models import sampled_protocol_inputs
+
+__all__ = ["evaluate_models", "find_optimal_svd_rank", "rank_sweep_lists", "set_config"]
+
+
+def set_config(model, config, convert_nan=True):
+    """pipelines.py:56-60: set every ``name: value`` of ``config`` as a model attribute (NaN -> None)."""
+    for name, value in config.items():
+        if convert_nan and value != value:
+            value = None
+        setattr(model, name, value)
+
+
+def evaluate_models(models, target_metric="precision", metric_type="all", **kwargs):
+    """pipelines.py:63-78: ``{model.method: target metric}`` of ``model.evaluate(metric_type, **kwargs)`` for one model or
+    a collection of them; ``target_metric`` is a metric name or a callable applied to the row of all metrics."""
+    import pandas as pd
+    if isinstance(models, (str, bytes, Mapping)) or not isinstance(models, Iterable):
+        models = [models]
+    out = {}
+    for model in models:
+        res = model.evaluate(metric_type, **kwargs)
+        row = pd.concat([pd.DataFrame([r]) for r in (res if isinstance(res, list) else [res])], axis=1)
+        if isinstance(target_metric, str):
+            value = row[target_metric]
+        elif callable(target_metric):
+            value = row.apply(target_metric, axis=1)
+        else:
+            raise NotImplementedError("target_metric must be a metric name or a callable")
+        out[model.method] = value.squeeze()
+    return out
+
+
+def rank_sweep_lists(model, ranks):
+    """``{rank: lists}`` of ``model.recommendations`` at every rank, from one sweep: the sampled protocol when the model
+    predicts holdout positions (``_prediction_target`` other than the item field; inputs read from the data model as
+    the sampled drop-in's ``get_recommendations`` reads them), the standard one otherwise."""
+    if model._prediction_target == model.data.fields.itemid:
+        return model.rank_sweep(ranks)
+    holdout_items, unseen, kwargs = sampled_protocol_inputs(model)
+    return model.sampled_rank_sweep(ranks, holdout_items, unseen, **kwargs)
+
+
+def find_optimal_svd_rank(model, ranks, target_metric, return_scores=False, protect_factors=True, config=None,
+                          verbose=False, evaluator=None, iterator=lambda x: x, **kwargs):
+    """pipelines.py:81-116 with the lists of all ranks from one device sweep (see the module docstring).  Returns the
+    rank with the best ``target_metric`` and, with ``return_scores``, the Series of scores in the order of ``ranks``.
+    ``evaluator(model, target_metric, **kwargs)`` defaults to :func:`evaluate_models`."""
+    import pandas as pd
+    evaluator = evaluator or evaluate_models
+    model_verbose = model.verbose
+    if config:
+        set_config(model, config)
+    svd_rank = max(max(ranks), model.rank)
+    model.rank = svd_rank
+    if not model._is_ready:
+        model.verbose = verbose
+        model.build()
+    if protect_factors:
+        svd_factors = dict(model.factors)
+    res = {}
+    try:
+        lists = rank_sweep_lists(model, ranks)
+        for rank in iterator(sorted(ranks, reverse=True)):
+            model.rank = rank
+            model._recommendations = lists[rank]
+            res[rank] = evaluator(model, target_metric, **kwargs)[model.method]
+            model._recommendations = None          # the next rank must not see this rank's lists
+    finally:
+        if protect_factors:
+            model._rank = svd_rank
+            model.factors = svd_factors
+        model.verbose = model_verbose
+    scores = pd.Series(res)
+    best_rank = scores.idxmax()
+    if return_scores:
+        scores.index.name = "rank"
+        scores.name = model.method
+        return best_rank, scores.loc[list(ranks)]
+    return best_rank
