@@ -318,6 +318,34 @@ int pb200_topk_dense(pb200_ctx* ctx, const void* S, int dtype, int64_t lds, int6
 int pb200_downvote_dense(pb200_ctx* ctx, void* S, int dtype, int64_t lds, int64_t m, int64_t n,
                          const int64_t* rows, const int64_t* cols, int64_t nnz);
 
+/* Item-to-item model (CooccurrenceModel, models.py:693-725).
+ * pb200_cooc_build: S = A^T A with a zero diagonal (models.py:702-709) as a DENSE fp64 matrix S [n x lds], n = a->n_cols.
+ *   `a` is the training CSR split into column panels of at most PB200_COOC_MAX_PANEL_BYTES / 8 columns
+ *   (pb200_csr_block_columns; one panel when it is narrow enough), `at` the plain CSR of A^T (pb200_csr_transpose).
+ *   implicit != 0 takes sign(a_ui) for every value (models.py:699-701).  Every entry is summed over the users in
+ *   ascending order; fp32 products are exact in fp64, so integer-valued data gives S exactly (and exactly symmetric). */
+#define PB200_COOC_MAX_PANEL_BYTES 196608
+int pb200_cooc_build(pb200_ctx* ctx, const pb200_csr_view* a, const pb200_csr_view* at, int implicit, double* S,
+                     int64_t lds);
+/* pb200_i2i_topk: for each of the m test users (CSR p_*, the test matrix of get_test_matrix, models.py:180-211)
+ * s_u = sum_i p_ui S[i, :] in fp64 with i ascending, a rounded product then a rounded sum (scipy's csr_matmat order;
+ * implicit != 0 takes sign(p_ui)), and
+ *   out_nnz    int64 [m]      |{j : s_uj != 0}| over all items, seen ones included;
+ *   out_dense  int64 [m x k]  the dense-chunk rule (toarray + downvote_seen_items + topsort, models.py:510-519, 561-563):
+ *                             unseen items by (score desc, id asc), zero scores included, then the seen ones in the same
+ *                             order; without a seen CSR every item by (score desc, id asc);
+ *   out_sparse int64 [m x k]  the sparse-chunk rule (models.py:524-560): the items with s != 0 by (score desc, id asc),
+ *                             seen ones included, then -1 up to k.  downvote_seen_items' sparse branch (models.py:
+ *                             501-509) has no effect on the caller's block: `recs -= seen_recs` rebinds a local name,
+ *                             scipy's sparse matrices having no in-place subtraction;
+ *   out_scores fp64 [m x k]   the scores of out_dense, or NULL.
+ * seen_*: int64 indptr [m+1] / sorted int32 ids of the seen items, or both NULL.  1 <= k <= n.  No [m x n] block is
+ * formed and each S row of a user is read once. */
+int pb200_i2i_topk(pb200_ctx* ctx, const double* S, int64_t lds, int64_t n, int64_t m, const int64_t* p_indptr,
+                   const int32_t* p_indices, const float* p_values, const int64_t* seen_indptr,
+                   const int32_t* seen_indices, int implicit, int k, int64_t* out_nnz, int64_t* out_dense,
+                   int64_t* out_sparse, double* out_scores);
+
 /* res[i0,:,:] += val * U[i1,:] (x) W[i2,:] over all nnz of a 3-way COO tensor sorted
  * and grouped by mode-0 index (CSR-like: seg_ptr int64 [n0+1], i1/i2 int32 [nnz]);
  * out [n0 x ru*rw] row-major (ld = ldo).  Replaces dttm_seq/dttm_par,

@@ -463,6 +463,45 @@ class Engine:
         self._check(st, "sampled_topk_ranks")
         return (pos, scores) if want_scores else pos
 
+    # columns of one build CTA's row panel of S (fp64 in shared memory: 64 KB, three CTAs per SM)
+    COOC_PANEL_COLS = 8192
+
+    def cooc_build(self, a: DeviceCSR, implicit=False, at=None):
+        """item-to-item matrix S = A^T A with a zero diagonal, fp64 [n_items x lds] (pb200_cooc_build); ``implicit`` takes
+        sign(a_ui).  Refuses with MemoryError, before allocating anything, when S and the build's scratch do not fit the
+        device's free memory (``cooc_memory_check``).  Returns ``S`` (its first n_items columns are the matrix)."""
+        m, n = a.shape
+        panel_cols = min(n, self.COOC_PANEL_COLS)
+        n_panels = -(-n // panel_cols)
+        scratch = (0 if at is not None else a.nbytes() + 8 * n) + (a.nbytes() + 8 * n_panels * m if n_panels > 1 else 0) \
+            + 32 * n
+        cooc_memory_check(n, scratch, torch.cuda.mem_get_info(self.device)[0])
+        if at is None:
+            at = self.transpose(a)
+        a_blk = self.block_columns(a, panel_cols)
+        lds = cooc_lds(n)
+        s = self.empty((n, lds), torch.float64)
+        va, vt = a_blk.view(), at.view()
+        st = self.lib.pb200_cooc_build(self.h, C.byref(va), C.byref(vt), int(bool(implicit)), _p(s, _F64), lds)
+        self._check(st, "cooc_build")
+        return s
+
+    def i2i_topk(self, s, n_items, p: DeviceCSR, k, seen=None, implicit=False, want_scores=False):
+        """per test user the nonzero count of ``P S`` and its top-k lists under the dense and the sparse chunk rule
+        (pb200_i2i_topk): returns ``(nnz int64 [m], dense int64 [m x k], sparse int64 [m x k])`` plus the fp64 scores of
+        the dense lists with ``want_scores``."""
+        m = p.shape[0]
+        nnz = self.empty((m,), torch.int64)
+        dense = self.empty((m, k), torch.int64)
+        sparse = self.empty((m, k), torch.int64)
+        scores = self.empty((m, k), torch.float64) if want_scores else None
+        sp, si = (seen if seen is not None else (None, None))
+        st = self.lib.pb200_i2i_topk(self.h, _p(s, _F64), s.stride(0), int(n_items), m, _p(p.indptr, _I64),
+                                     _p(p.indices, _I32), _p(p.values, _F32), _p(sp, _I64), _p(si, _I32),
+                                     int(bool(implicit)), int(k), _p(nnz), _p(dense), _p(sparse), _p(scores))
+        self._check(st, "i2i_topk")
+        return (nnz, dense, sparse, scores) if want_scores else (nnz, dense, sparse)
+
     def score_dense(self, e, v, r):
         m, n = e.shape[0], v.shape[0]
         s = self.empty((m, n))
@@ -515,6 +554,23 @@ class Engine:
                                        a.stride(0), _p(b, _F32), rb, b.stride(0), _p(out), ra * rb)
         self._check(st, "ttm_reduce")
         return out
+
+
+def cooc_lds(n_items):
+    """row stride of the dense item-to-item matrix: rows start on 128-byte boundaries."""
+    return round_up(int(n_items), 16)
+
+
+def cooc_memory_check(n_items, scratch_bytes, free_bytes):
+    """Raises MemoryError when the dense fp64 item-to-item matrix of ``n_items`` items plus ``scratch_bytes`` exceeds
+    ``free_bytes`` (the device's free memory); storing S sparsely for larger catalogues is not implemented."""
+    need_s = int(n_items) * cooc_lds(n_items) * 8
+    need = need_s + int(scratch_bytes)
+    if need > int(free_bytes):
+        raise MemoryError("item-to-item model: the dense item x item matrix of %d items takes %d bytes (plus %d bytes of "
+                          "scratch, %d in all), but only %d bytes of device memory are free"
+                          % (int(n_items), need_s, int(scratch_bytes), need, int(free_bytes)))
+    return need
 
 
 _ENGINES = {}

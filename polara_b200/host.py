@@ -102,10 +102,12 @@ Experience = namedtuple("Experience", "coverage")
 
 
 def _match_holdout(recs, h_user, h_item):
-    """rank (1-based) at which each holdout row appears in its user's list, 0 = absent."""
+    """rank (1-based) at which each holdout row appears in its user's list, 0 = absent.  Negative entries (the -1 pads
+    of lists shorter than k) are no recommendation, as in build_rank_matrix (evaluation.py:29-36)."""
     m, k = recs.shape
     n_items = int(max(recs.max(), h_item.max())) + 1
     rec_key = (np.repeat(np.arange(m, dtype=np.int64), k) * n_items + recs.ravel().astype(np.int64))
+    rec_key[recs.ravel() < 0] = -1
     order = np.argsort(rec_key, kind="stable")
     sorted_key = rec_key[order]
     hold_key = h_user.astype(np.int64) * n_items + h_item.astype(np.int64)

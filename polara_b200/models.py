@@ -22,7 +22,8 @@ import torch
 from . import host
 from .engine import DeviceCSR, get_engine, round_up
 
-__all__ = ["B200SVDModel", "B200ScaledSVD", "B200CoffeeModel", "dropin", "default_ell"]
+__all__ = ["B200SVDModel", "B200ScaledSVD", "B200CoffeeModel", "B200CooccurrenceModel", "dropin", "dropin_i2i",
+           "default_ell"]
 
 
 def default_ell(rank, oversample=None):
@@ -1038,6 +1039,115 @@ class B200CoffeeModel(_CoffeeDeviceMixin, host.RecommenderModel):
 
     def build(self):
         return _CoffeeDeviceMixin.build(self)
+
+
+# ------------------------------------------------------------------ item-to-item ----------
+def cooc_nnz_max(memory_hard_limit):
+    """``get_nnz_max`` (lib/sparse.py:21-22): beyond this many stored scores a chunk's sparse block is made dense."""
+    import sys
+    per_entry = sys.getsizeof(()) + 2 * (sys.getsizeof(1.0) + np.dtype(np.intp).itemsize)
+    return int(memory_hard_limit * (1024 ** 3) / per_entry)
+
+
+def cooc_chunk_modes(nnz_u, n_items, topk, memory_hard_limit, dense_output=False):
+    """The reference's user chunks for the item-to-item model and the form each chunk's score block takes there:
+    ``[(start, stop, dense)]``.  Chunks: ``array_split`` (utils.py:7-53) with result width ``topk``, scores multiplier 1
+    and float64 scores; ``get_available_memory()`` returns bytes that are read as GB, so the limit is exactly
+    ``memory_hard_limit`` whenever it is set (and never binds otherwise).  Form (lib/sparse.py:25-55): dense with
+    ``dense_output``, or when the chunk's nonzero scores ``sum(nnz_u)`` exceed ``cooc_nnz_max`` or half the block."""
+    nnz_u = np.asarray(nnz_u, dtype=np.int64)
+    m, n = int(nnz_u.shape[0]), int(n_items)
+    chunk = m
+    s0, s1 = m / 1024, n / 1024
+    item_kb = np.dtype(np.float64).itemsize / 1024
+    result_mem = s0 * (topk / 1024) * item_kb
+    if memory_hard_limit and s0 * s1 * item_kb + result_mem > memory_hard_limit:
+        chunk = min(int((memory_hard_limit - result_mem) / (s1 * item_kb * (1 / 1024) + item_kb / 1024 ** 2) - 1), chunk)
+        if chunk <= 0:
+            raise MemoryError()
+    n_chunks = m // chunk + int(m % chunk > 0)
+    size, rem = divmod(m, n_chunks)
+    bounds = np.cumsum([0] + rem * [size + 1] + (n_chunks - rem) * [size])
+    nnz_max = cooc_nnz_max(memory_hard_limit)
+    out = []
+    for a, b in zip(bounds[:-1].tolist(), bounds[1:].tolist()):
+        nnz = int(nnz_u[a:b].sum())
+        out.append((a, b, bool(dense_output or nnz > nnz_max or nnz > 0.5 * (b - a) * n)))
+    return out
+
+
+class _CooccurrenceDeviceMixin(_DeviceModelMixin):
+    """Device implementation of CooccurrenceModel.build / get_recommendations (models.py:693-725, 391-405): S = A^T A
+    stays on the device as a dense fp64 matrix; scoring computes every test user's ``P S`` row once and returns its list
+    under the rule the reference's chunk of that user applies (``cooc_chunk_modes``)."""
+
+    def _memory_hard_limit(self):
+        return host.DEFAULTS["memory_hard_limit"]
+
+    def build(self):
+        data = self.data
+        idx, val, shape = data.to_coo(tensor_mode=False, feedback_threshold=self.feedback_threshold)
+        eng = self.engine
+        t0 = time.perf_counter()
+        idx_d = eng.upload(np.ascontiguousarray(_as_index_array(idx)))
+        a = eng.coo_to_csr(idx_d[:, 0], idx_d[:, 1], eng.upload(_as_value_array(val)), shape)
+        self._i2i_dev = eng.cooc_build(a, implicit=self.implicit)
+        self._i2i_items = int(shape[1])
+        eng.sync()
+        t1 = time.perf_counter()
+        if self.training_time is not None:
+            self.training_time.append(t1 - t0)          # track_time, models.py:703
+        if self.verbose:
+            print("{} training time: {:.3f}s".format(self.method, t1 - t0))
+
+    def get_recommendations(self):
+        if self.verify_integrity and hasattr(self, "verify_data_integrity"):
+            self.verify_data_integrity()
+        test_data, shape, _ = self._get_test_data()
+        if self.topk > shape[1]:
+            raise ValueError("topk exceeds the number of items")
+        nnz, dense, sparse = self.i2i_lists(test_data, shape)
+        out = np.empty((shape[0], self.topk), dtype=np.int64)
+        for a, b, is_dense in cooc_chunk_modes(nnz, shape[1], self.topk, self._memory_hard_limit(), self.dense_output):
+            out[a:b] = dense[a:b] if is_dense else sparse[a:b]
+        return out
+
+    def i2i_lists(self, test_data, shape):
+        """``(nnz_u, dense-rule lists, sparse-rule lists)`` of the test users, as numpy arrays (pb200_i2i_topk)."""
+        eng = self.engine
+        p_dev, seen_dev = self._test_csr_device(test_data, shape)
+        nnz, dense, sparse = eng.i2i_topk(self._i2i_dev, self._i2i_items, p_dev, self.topk,
+                                          seen=seen_dev if self.filter_seen else None, implicit=self.implicit)
+        return nnz.cpu().numpy(), dense.cpu().numpy(), sparse.cpu().numpy()
+
+
+class B200CooccurrenceModel(_CooccurrenceDeviceMixin, host.RecommenderModel):
+    """Stand-alone item-to-item model (CooccurrenceModel, models.py:693-725)."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.method = "item-to-item"
+        self.implicit = False
+        self.dense_output = False
+
+    def build(self):
+        return _CooccurrenceDeviceMixin.build(self)
+
+
+def dropin_i2i():
+    """``PolaraB200Cooccurrence``: the device item-to-item model on the REAL ``polara`` CooccurrenceModel; the chunk
+    rules read ``polara.recommender.defaults.memory_hard_limit`` as the reference does."""
+    from polara.recommender import defaults
+    from polara.recommender.models import CooccurrenceModel
+
+    class PolaraB200Cooccurrence(_CooccurrenceDeviceMixin, CooccurrenceModel):
+        def _memory_hard_limit(self):
+            return defaults.memory_hard_limit
+
+        def build(self):
+            return _CooccurrenceDeviceMixin.build(self)
+
+    return PolaraB200Cooccurrence
 
 
 def dropin():
