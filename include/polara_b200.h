@@ -193,6 +193,20 @@ int pb200_rsvd_csr(pb200_ctx* ctx, const pb200_csr_view* A, const pb200_csr_view
                    int rank, int ell, int max_iters, double tol, double vec_tol, uint64_t seed,
                    float* V_out, int64_t ldv, double* sigma_out, float* U_out, int64_t ldu, double* info_host);
 
+/* The same factorisation of the matrix-free operator M = K_u^T A K_i (HybridSVD, hybrid/models.py:368-384): every
+ * product of the subspace iteration and of the Rayleigh-Ritz step is the chain
+ *   M X = K_u^T (A (K_i X))        M^T W = K_i^T (A^T (K_u W))
+ * of SpMMs, so V_out / sigma_out / U_out are the right vectors, singular values and left vectors of M.  Each factor is a
+ * pair of views (K, K^T), plain or panel-major; a NULL pair is the identity on that side (both NULL = pb200_rsvd_csr).
+ * K_i, K_i^T are n_cols x n_cols and K_u, K_u^T n_rows x n_rows (A is n_rows x n_cols), else PB200_EINVAL.  Factors
+ * under a reduce hook return PB200_ENOTIMPL: a user factor mixes rows of different shards.  Scratch: two more panels,
+ * [n_cols x ell] and [n_rows x ell], when a factor is given. */
+int pb200_rsvd_factored(pb200_ctx* ctx, const pb200_csr_view* A, const pb200_csr_view* At,
+                        const pb200_csr_view* Ki, const pb200_csr_view* Kit,
+                        const pb200_csr_view* Ku, const pb200_csr_view* Kut,
+                        int rank, int ell, int max_iters, double tol, double vec_tol, uint64_t seed,
+                        float* V_out, int64_t ldv, double* sigma_out, float* U_out, int64_t ldu, double* info_host);
+
 /* Thin SVD pieces of a dense tall matrix M [n x c]: leading `rank` singular values
  * (sigma_out, float64, descending), left vectors U_out [n x ldu] and, if not NULL,
  * right vectors Vt_out [rank x c] (row-major).  Replaces svds() on the dense HOOI

@@ -48,6 +48,9 @@ _SIGNATURES = {
     "pb200_csr_block_columns": ([ptr, i64, i64, i64, ptr, ptr, ptr, i64, C.c_int, ptr, ptr, ptr, ptr], C.c_int),
     "pb200_rsvd_csr": ([ptr, C.POINTER(CsrView), C.POINTER(CsrView), C.c_int, C.c_int, C.c_int, f64, f64, C.c_uint64,
                         ptr, i64, ptr, ptr, i64, C.POINTER(f64)], C.c_int),
+    "pb200_rsvd_factored": ([ptr, C.POINTER(CsrView), C.POINTER(CsrView), C.POINTER(CsrView), C.POINTER(CsrView),
+                             C.POINTER(CsrView), C.POINTER(CsrView), C.c_int, C.c_int, C.c_int, f64, f64, C.c_uint64,
+                             ptr, i64, ptr, ptr, i64, C.POINTER(f64)], C.c_int),
     "pb200_spmm": ([ptr, i64, i64, i64, ptr, ptr, ptr, ptr, i64, ptr, i64, C.c_int], C.c_int),
     "pb200_csr_transpose": ([ptr, i64, i64, i64, ptr, ptr, ptr, ptr, ptr, ptr], C.c_int),
     "pb200_rescale": ([ptr, i64, i64, i64, ptr, ptr, ptr, f64, f64], C.c_int),

@@ -13,6 +13,9 @@
 // on the item side (Omega, Q, eig, V, sigma) is computed redundantly and identically on every rank; U_out holds the
 // rank's own rows.
 //
+// Factored operator (HybridSVD, pb200_rsvd_factored): A above stands for M = K_u^T A K_i, each product with M or M^T a
+// chain of up to three SpMMs through two extra panels; the iteration itself is unchanged.
+//
 // All SpMMs are fp32 (spmm.cu); Gram matrices and the small eigenproblems are fp64.
 #include <algorithm>
 #include <cmath>
@@ -51,19 +54,49 @@ __global__ void rows_to_float_kernel(const double* __restrict__ vecs, int c, int
 
 }  // namespace
 
-extern "C" int pb200_rsvd_csr(pb200_ctx* ctx, const pb200_csr_view* A, const pb200_csr_view* At,
-                              int rank, int ell, int max_iters, double tol, double vec_tol, uint64_t seed,
-                              float* V_out, int64_t ldv, double* sigma_out, float* U_out, int64_t ldu,
-                              double* info_host) {
+// One product of the operator chain  Y = Last (Mid (First X))  with First / Last optional (NULL = identity): the
+// subspace iteration of the factored operator M = K_u^T A K_i applies  M X = K_u^T (A (K_i X))  and
+// M^T W = K_i^T (A^T (K_u W)).  tmp_first holds First X (rows of Mid's column space), tmp_mid holds Mid (...) when Last
+// follows.  Every product is one SpMM (pb_spmm_view), so an identity factor (one unit nnz per row) copies exactly.
+static int apply_chain(pb200_ctx* ctx, const pb200_csr_view* first, const pb200_csr_view* mid, const pb200_csr_view* last,
+                       const float* X, float* tmp_first, float* tmp_mid, float* Y, int ell) {
+    if (first) {
+        PB_TRY(pb_spmm_view(ctx, first, X, ell, tmp_first, ell, ell));
+        X = tmp_first;
+    }
+    if (!last) return pb_spmm_view(ctx, mid, X, ell, Y, ell, ell);
+    PB_TRY(pb_spmm_view(ctx, mid, X, ell, tmp_mid, ell, ell));
+    return pb_spmm_view(ctx, last, tmp_mid, ell, Y, ell, ell);
+}
+
+extern "C" int pb200_rsvd_factored(pb200_ctx* ctx, const pb200_csr_view* A, const pb200_csr_view* At,
+                                   const pb200_csr_view* Ki, const pb200_csr_view* Kit,
+                                   const pb200_csr_view* Ku, const pb200_csr_view* Kut,
+                                   int rank, int ell, int max_iters, double tol, double vec_tol, uint64_t seed,
+                                   float* V_out, int64_t ldv, double* sigma_out, float* U_out, int64_t ldu,
+                                   double* info_host) {
     PB_ENTER(ctx);
     PB_REQUIRE(ctx, A && At && A->indptr && At->indptr, "rsvd: null matrix view");
     const int64_t n_rows = A->n_rows, n_cols = A->n_cols;
     PB_REQUIRE(ctx, At->n_rows == n_cols && At->n_cols == n_rows && At->nnz == A->nnz, "rsvd: A^T does not match A");
+    PB_REQUIRE(ctx, !Ki == !Kit && !Ku == !Kut, "rsvd: a factor needs both K and K^T (or neither)");
+    PB_REQUIRE(ctx, !Ki || (Ki->indptr && Kit->indptr && Ki->n_rows == n_cols && Ki->n_cols == n_cols &&
+                            Kit->n_rows == n_cols && Kit->n_cols == n_cols && Kit->nnz == Ki->nnz),
+               "rsvd: the item factor K_i and K_i^T must be n_cols x n_cols (n_cols of A) with equal nnz");
+    PB_REQUIRE(ctx, !Ku || (Ku->indptr && Kut->indptr && Ku->n_rows == n_rows && Ku->n_cols == n_rows &&
+                            Kut->n_rows == n_rows && Kut->n_cols == n_rows && Kut->nnz == Ku->nnz),
+               "rsvd: the user factor K_u and K_u^T must be n_rows x n_rows (n_rows of A) with equal nnz");
+    if ((Ki || Ku) && ctx->reduce_fn) {
+        ctx->err = "rsvd: factored operator under a reduce hook (row-sharded build) is not implemented: a user factor "
+                   "mixes the rows of all shards";
+        return PB200_ENOTIMPL;
+    }
     PB_REQUIRE(ctx, rank > 0 && ell % 32 == 0 && ell >= rank && ell <= 1024, "rsvd: need 0 < rank <= ell <= 1024, ell % 32 == 0");
     PB_REQUIRE(ctx, rank <= n_cols && (rank <= n_rows || ctx->reduce_fn), "rsvd: rank exceeds matrix dimension");
     PB_REQUIRE(ctx, ldv >= rank && (!U_out || ldu >= rank), "rsvd: leading dimension smaller than rank");
     Scratch sc(ctx);
     float *Yn = nullptr, *Qn = nullptr, *Qprev = nullptr, *Ym = nullptr, *Wm = nullptr, *Wsmall = nullptr;
+    float *Pi = nullptr, *Pu = nullptr;      // chain intermediates: item-side [n_cols x ell], user-side [n_rows x ell]
     double *lam = nullptr, *G = nullptr, *vecs = nullptr, *Cx = nullptr;
     PB_TRY(sc.alloc(&Yn, (size_t)n_cols * ell));
     PB_TRY(sc.alloc(&Qn, (size_t)n_cols * ell));
@@ -75,6 +108,10 @@ extern "C" int pb200_rsvd_csr(pb200_ctx* ctx, const pb200_csr_view* A, const pb2
     PB_TRY(sc.alloc(&G, (size_t)ell * ell));
     PB_TRY(sc.alloc(&vecs, (size_t)ell * ell));
     PB_TRY(sc.alloc(&Cx, (size_t)rank * rank));
+    if (Ki || Ku) {
+        PB_TRY(sc.alloc(&Pi, (size_t)n_cols * ell));
+        PB_TRY(sc.alloc(&Pu, (size_t)n_rows * ell));
+    }
     std::vector<double> prev(rank, 0.0), cur(ell, 0.0), cross((size_t)rank * rank, 0.0);
 
     PB_TRY(pb_fill_gaussian(ctx, Qn, n_cols * (int64_t)ell, seed));
@@ -82,9 +119,9 @@ extern "C" int pb200_rsvd_csr(pb200_ctx* ctx, const pb200_csr_view* A, const pb2
     double worst = 1.0, angle = 1.0;
     bool converged = false;
     for (int it = 0; it <= max_iters; ++it) {
-        PB_TRY(pb_spmm_view(ctx, A, Qn, ell, Ym, ell, ell));
+        PB_TRY(apply_chain(ctx, Ki, A, Kut, Qn, Pi, Pu, Ym, ell));                     // M Q
         PB_TRY(pb_orthonormalize(ctx, Ym, n_rows, ell, ell, Wm, ell, nullptr, /*rows_sharded=*/true));
-        PB_TRY(pb_spmm_view(ctx, At, Wm, ell, Yn, ell, ell));
+        PB_TRY(apply_chain(ctx, Ku, At, Kit, Wm, Pu, Pi, Yn, ell));                    // M^T W
         PB_TRY(pb_reduce(ctx, Yn, n_cols * (int64_t)ell, PB200_F32));     // A^T W = sum over row shards of A_g^T W_g
         std::swap(Qn, Qprev);
         PB_TRY(pb_orthonormalize(ctx, Yn, n_cols, ell, ell, Qn, ell, lam));
@@ -114,8 +151,8 @@ extern "C" int pb200_rsvd_csr(pb200_ctx* ctx, const pb200_csr_view* A, const pb2
         }
         if (it > 0 && worst < tol && angle <= std::max(vec_tol, 0.0)) { converged = true; break; }
     }
-    // Rayleigh-Ritz on the final subspace
-    PB_TRY(pb_spmm_view(ctx, A, Qn, ell, Ym, ell, ell));
+    // Rayleigh-Ritz on the final subspace: B = M Q (U = B Z / sigma are the left vectors of M)
+    PB_TRY(apply_chain(ctx, Ki, A, Kut, Qn, Pi, Pu, Ym, ell));
     PB_TRY(pb_gram(ctx, Ym, n_rows, ell, ell, G));
     PB_TRY(pb_reduce(ctx, G, (int64_t)ell * ell, PB200_F64));
     PB_TRY(pb_eig_psd(ctx, G, ell, lam, vecs));
@@ -134,6 +171,14 @@ extern "C" int pb200_rsvd_csr(pb200_ctx* ctx, const pb200_csr_view* A, const pb2
         for (int i = 4; i < 8; ++i) info_host[i] = 0.0;
     }
     return PB200_OK;
+}
+
+extern "C" int pb200_rsvd_csr(pb200_ctx* ctx, const pb200_csr_view* A, const pb200_csr_view* At,
+                              int rank, int ell, int max_iters, double tol, double vec_tol, uint64_t seed,
+                              float* V_out, int64_t ldv, double* sigma_out, float* U_out, int64_t ldu,
+                              double* info_host) {
+    return pb200_rsvd_factored(ctx, A, At, nullptr, nullptr, nullptr, nullptr, rank, ell, max_iters, tol, vec_tol, seed,
+                               V_out, ldv, sigma_out, U_out, ldu, info_host);
 }
 
 extern "C" int pb200_rsvd(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, int64_t nnz,

@@ -309,17 +309,37 @@ class Engine:
                                     _p(a.values), float(row_scaling), float(col_scaling))
         self._check(st, "rescale")
 
-    def rsvd(self, a: DeviceCSR, at: DeviceCSR, rank, ell, max_iters=8, tol=1e-6, seed=1, want_u=False, vec_tol=0.0):
+    def rsvd(self, a: DeviceCSR, at: DeviceCSR, rank, ell, max_iters=8, tol=1e-6, seed=1, want_u=False, vec_tol=0.0,
+             item_factor=None, user_factor=None):
         """returns (V, sigma, U | None, iters); convergence details of the call are left in ``self.last_rsvd_info``:
-        ``dict(iters, value_change, angle_bound, converged)`` (see pb200_rsvd_csr)."""
+        ``dict(iters, value_change, angle_bound, converged)`` (see pb200_rsvd_csr).
+
+        ``item_factor`` / ``user_factor``: ``(K, K^T)`` pairs of DeviceCSR; with either the factorised operator is the
+        matrix-free ``K_u^T A K_i`` (pb200_rsvd_factored), a missing side being the identity.  A factor whose gathered
+        operand (its column count x ``ell`` floats) exceeds ``PANEL_BYTES`` is stored panel-major (``block_columns``)
+        for the call, as the caller does for A and A^T."""
         ldv = round_up(rank, 32)
         v = self.zeros((a.shape[1], ldv))
         sigma = self.empty((rank,), torch.float64)
         u = self.zeros((a.shape[0], ldv)) if want_u else None
         info = (C.c_double * 8)()
         va, vt = a.view(), at.view()
-        st = self.lib.pb200_rsvd_csr(self.h, C.byref(va), C.byref(vt), rank, ell, max_iters, float(tol), float(vec_tol),
-                                     int(seed), _p(v), ldv, _p(sigma), _p(u), ldv, info)
+        if item_factor is None and user_factor is None:
+            st = self.lib.pb200_rsvd_csr(self.h, C.byref(va), C.byref(vt), rank, ell, max_iters, float(tol),
+                                         float(vec_tol), int(seed), _p(v), ldv, _p(sigma), _p(u), ldv, info)
+        else:
+            keep, views = [], []
+            for pair in (item_factor, user_factor):
+                for k in (pair if pair is not None else (None, None)):
+                    if k is None:
+                        views.append(None)
+                        continue
+                    k = self.block_columns(k, self.panel_cols_for(k.shape[1], ell))
+                    keep.append(k)                     # the views hold raw pointers into these
+                    views.append(C.byref(k.view()))
+            st = self.lib.pb200_rsvd_factored(self.h, C.byref(va), C.byref(vt), *views, rank, ell, max_iters,
+                                              float(tol), float(vec_tol), int(seed), _p(v), ldv, _p(sigma), _p(u), ldv,
+                                              info)
         self._check(st, "rsvd")
         self.last_rsvd_info = dict(iters=int(info[0]), value_change=float(info[1]), angle_bound=float(info[2]),
                                    converged=bool(info[3]))

@@ -22,8 +22,8 @@ import torch
 from . import host
 from .engine import DeviceCSR, get_engine, round_up
 
-__all__ = ["B200SVDModel", "B200ScaledSVD", "B200CoffeeModel", "B200CooccurrenceModel", "dropin", "dropin_i2i",
-           "default_ell"]
+__all__ = ["B200SVDModel", "B200ScaledSVD", "B200HybridSVD", "B200ScaledHybridSVD", "B200CoffeeModel",
+           "B200CooccurrenceModel", "dropin", "dropin_hybrid", "dropin_i2i", "default_ell"]
 
 
 def default_ell(rank, oversample=None):
@@ -240,11 +240,13 @@ class _SVDDeviceMixin(_DeviceModelMixin):
             if sharded:
                 eng.set_reduce_hook(None)
 
-    def _build_factors(self, eng, return_factors, sharded, op_csr=None):
+    def _build_factors(self, eng, return_factors, sharded, op_csr=None, a=None, item_factor=None, user_factor=None):
+        """``a``: the training matrix already on the device; ``item_factor`` / ``user_factor``: ``(K, K^T)`` DeviceCSR pairs
+        of a factored operator ``K_u^T A K_i`` (Engine.rsvd)."""
         t0 = time.perf_counter()
-        if op_csr is None:
+        if a is None and op_csr is None:
             a = self._training_csr_device()
-        else:
+        elif a is None:
             a = eng.upload_csr(op_csr.indptr.astype(np.int64), op_csr.indices.astype(np.int32),
                                op_csr.data.astype(np.float32), op_csr.shape)
             self._n_train_users = op_csr.shape[0]
@@ -260,7 +262,8 @@ class _SVDDeviceMixin(_DeviceModelMixin):
         eng.sync()
         t1 = time.perf_counter()
         v, sigma, u, iters = eng.rsvd(a, at, rank, ell, max_iters=self.power_iters, tol=self.tol, vec_tol=self.vec_tol,
-                                      seed=self.rsvd_seed, want_u=want_u)
+                                      seed=self.rsvd_seed, want_u=want_u, item_factor=item_factor,
+                                      user_factor=user_factor)
         eng.sync()
         info = dict(eng.last_rsvd_info)
         if not info["converged"]:
@@ -810,8 +813,9 @@ class B200SVDModel(_SVDDeviceMixin, _SVDState, host.RecommenderModel):
         return _SVDDeviceMixin.build(self, operator=operator, return_factors=return_factors)
 
 
-class B200ScaledSVD(B200SVDModel):
-    """ScaledMatrixMixin + SVDModel (models.py:864-898)."""
+class _ScaledMatrixMixin:
+    """ScaledMatrixMixin (models.py:864-895): column / row scaling of the training matrix, applied on the device by
+    ``_SVDDeviceMixin._scaled``."""
 
     def __init__(self, *args, **kwargs):
         super().__init__(*args, **kwargs)
@@ -838,6 +842,158 @@ class B200ScaledSVD(B200SVDModel):
         if new_value != self._row_scaling:
             self._row_scaling = new_value
             self._recommendations = None
+
+
+class B200ScaledSVD(_ScaledMatrixMixin, B200SVDModel):
+    """ScaledMatrixMixin + SVDModel (models.py:864-898)."""
+
+
+# ------------------------------------------------------------------ HybridSVD ----------
+def cholesky_factor_parts(factor):
+    """``(L, perm)`` of a Cholesky factor ``K = P^T L`` of a similarity matrix, ``L L^T = P (S + beta I) P^T``: polara's
+    ``CholeskyFactor`` (lib/cholesky.py; ``.L`` and the CHOLMOD factor's ``P()``) or an ``(L, perm)`` pair.  ``L`` comes
+    back as a float64 CSR with sorted indices, ``perm`` as int64.  None stays None (that side is the identity)."""
+    if factor is None:
+        return None
+    import scipy.sparse as sps_
+    if isinstance(factor, (tuple, list)):
+        lower, perm = factor
+    else:
+        lower, perm = factor.L, factor._factor.P()
+    lower = sps_.csr_matrix(lower, dtype=np.float64)
+    lower.sum_duplicates()
+    lower.sort_indices()
+    perm = np.asarray(perm, dtype=np.int64).ravel()
+    n = lower.shape[0]
+    if lower.shape[1] != n or perm.shape[0] != n or not np.array_equal(np.sort(perm), np.arange(n)):
+        raise ValueError("a Cholesky factor needs a square L and a permutation of its %d rows; got L %s and %d entries"
+                         % (n, lower.shape, perm.shape[0]))
+    return lower, perm
+
+
+def cholesky_operator(lower, perm):
+    """the CSR of ``K = P^T L`` (host, float64): ``K v = apply_Pt(L v)`` puts row i of ``L`` at row ``perm[i]``."""
+    inv = np.empty_like(perm)
+    inv[perm] = np.arange(perm.shape[0], dtype=perm.dtype)
+    k = lower[inv]
+    k.sort_indices()
+    return k
+
+
+def hybrid_item_projectors(lower, perm, v):
+    """build_item_projector (hybrid/models.py:315-326) in float64 on the host: ``(left, right) = (K^-T v, K v)`` with
+    ``K^-T v = apply_Pt(L^-T v)`` (``chol.T.solve``, a triangular solve with ``L^T``) and ``K v = apply_Pt(L v)``
+    (``chol.dot``).  Runs once per build."""
+    from scipy.sparse.linalg import spsolve_triangular
+    v = np.asarray(v, dtype=np.float64)
+    right = np.empty_like(v)
+    right[perm] = lower @ v
+    left = np.empty_like(v)
+    left[perm] = spsolve_triangular(lower.T.tocsr(), v, lower=False)
+    return left, right
+
+
+def _rescale_host(matrix, scaling, axis):
+    """rescale_matrix (preprocessing/matrices.py:71-93, binary=True) on a float64 CSR: the lines along ``axis`` scaled by
+    ``sqrt(nnz count) ** (scaling - 1)``."""
+    import scipy.sparse as sps_
+    if scaling == 1:
+        return matrix
+    norm = np.sqrt(np.asarray(matrix.getnnz(axis=axis)).ravel().astype(np.float64))
+    factor = np.ones_like(norm)
+    factor[norm != 0] = np.power(norm[norm != 0], scaling - 1)
+    d = sps_.diags(factor)
+    return (matrix @ d).tocsr() if axis == 0 else (d @ matrix).tocsr()
+
+
+class _HybridSVDDeviceMixin(_SVDDeviceMixin):
+    """Device implementation of HybridSVD.build (hybrid/models.py:352-388): the truncated SVD of ``K_u^T A K_i`` for the
+    Cholesky factors ``K = P^T L`` of the user and item similarity matrices (either may be None: identity).  Without
+    ``precompute_auxiliary_matrix`` the operator is never formed: the subspace iteration applies the three factors in
+    turn (pb200_rsvd_factored); with it the product is formed on the host by scipy and factorised as an explicit
+    operator (``build(operator=...)``).  The item projectors of the scoring step are then computed on the host in
+    float64, as the reference computes them."""
+
+    def _host_training_matrix(self):
+        """get_training_matrix(dtype=np.float64) (models.py:160-177, 891-895 for the scaled variant) as a float64 CSR."""
+        getter = getattr(self, "get_training_matrix", None)
+        if getter is not None:
+            return getter(dtype=np.float64)
+        import scipy.sparse as sps_
+        idx, val, shape = self.data.to_coo(tensor_mode=False, feedback_threshold=self.feedback_threshold)
+        idx = _as_index_array(idx)
+        m = sps_.coo_matrix((np.asarray(val, dtype=np.float64), (idx[:, 0], idx[:, 1])), shape=shape).tocsr()
+        if hasattr(self, "_col_scaling"):
+            m = _rescale_host(_rescale_host(m, self.row_scaling, 1), self.col_scaling, 0)
+        return m
+
+    def _device_factor_pair(self, lower, perm):
+        """``(K, K^T)`` on the device: K formed on the host from L and perm (float32 values), K^T by pb200_csr_transpose."""
+        eng = self.engine
+        k = cholesky_operator(lower, perm)
+        k_dev = eng.upload_csr(k.indptr.astype(np.int64), k.indices.astype(np.int32), k.data.astype(np.float32), k.shape)
+        return k_dev, eng.transpose(k_dev)
+
+    def build(self, return_factors="vh"):
+        if not getattr(self, "_sparse_mode", True):
+            raise NotImplementedError("Check the installation of scikit-sparse package.")
+        if self._build_rows(1) is not None:
+            raise NotImplementedError("row-sharded build of HybridSVD")
+        # the order matters, as in the reference: reading the training data may fire the data model's change events,
+        # which reset the Cholesky factors
+        if self.precompute_auxiliary_matrix:
+            svd_matrix = self._host_training_matrix()
+        else:
+            a = self._training_csr_device()
+        items = cholesky_factor_parts(self.item_cholesky_factor)
+        users = cholesky_factor_parts(self.user_cholesky_factor)
+        if self.precompute_auxiliary_matrix:
+            if items is not None:
+                svd_matrix = (svd_matrix @ cholesky_operator(*items)).tocsr()
+            if users is not None:
+                svd_matrix = (cholesky_operator(*users).T @ svd_matrix).tocsr()
+            _SVDDeviceMixin.build(self, operator=svd_matrix, return_factors=return_factors)
+        else:
+            item_pair = None if items is None else self._device_factor_pair(*items)
+            user_pair = None if users is None else self._device_factor_pair(*users)
+            self._build_factors(self.engine, return_factors, False, a=a, item_factor=item_pair, user_factor=user_pair)
+        self.build_item_projector(self.factors[self.data.fields.itemid])
+        self._clear_cholesky_cache()
+
+    def build_item_projector(self, v):
+        items = cholesky_factor_parts(self.item_cholesky_factor)
+        if items is not None:
+            itemid = self.data.fields.itemid
+            left, right = hybrid_item_projectors(items[0], items[1], v)
+            self.factors["%s_projector_left" % itemid] = left
+            self.factors["%s_projector_right" % itemid] = right
+
+
+class B200HybridSVD(_HybridSVDDeviceMixin, _SVDState, host.RecommenderModel):
+    """Stand-alone HybridSVD (hybrid/models.py:335-394).  ``item_cholesky_factor`` / ``user_cholesky_factor``: polara's
+    ``CholeskyFactor`` or an ``(L, perm)`` pair with ``L L^T = P (S + beta I) P^T`` and ``P v = v[perm]``; None (the
+    default) leaves that side of the operator the identity.  Computing the factorisation is the caller's."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self._init_svd_state()
+        self.method = "HybridSVD"
+        self.precompute_auxiliary_matrix = False
+        self.item_cholesky_factor = None
+        self.user_cholesky_factor = None
+
+    def build(self, return_factors="vh"):
+        return _HybridSVDDeviceMixin.build(self, return_factors=return_factors)
+
+    def _clear_cholesky_cache(self):
+        """hybrid/models.py:241-247: a CholeskyFactor drops its cached L (an ``(L, perm)`` pair is the caller's)."""
+        for factor in (self.item_cholesky_factor, self.user_cholesky_factor):
+            if factor is not None and hasattr(factor, "_L"):
+                factor._L = None
+
+
+class B200ScaledHybridSVD(_ScaledMatrixMixin, B200HybridSVD):
+    """ScaledHybridSVD (hybrid/models.py:397): HybridSVD on the scaled training matrix."""
 
 
 # ------------------------------------------------------------------ CoFFee ----------
@@ -1168,6 +1324,24 @@ def dropin():
             return _CoffeeDeviceMixin.build(self)
 
     return PolaraB200SVD, PolaraB200ScaledSVD, PolaraB200Coffee
+
+
+def dropin_hybrid():
+    """``(PolaraB200HybridSVD, PolaraB200ScaledHybridSVD)``: the device HybridSVD build on the REAL ``polara`` HybridSVD
+    and ScaledHybridSVD (hybrid/models.py:335-397).  The Cholesky factors come from polara's own CholeskyFactorsMixin
+    (CHOLMOD on the host); the build follows HybridSVD.build, with the matrix-free operator on the device
+    (pb200_rsvd_factored)."""
+    from polara.recommender.hybrid.models import HybridSVD, ScaledHybridSVD
+
+    class PolaraB200HybridSVD(_HybridSVDDeviceMixin, HybridSVD):
+        def build(self, return_factors="vh"):
+            return _HybridSVDDeviceMixin.build(self, return_factors=return_factors)
+
+    class PolaraB200ScaledHybridSVD(_HybridSVDDeviceMixin, ScaledHybridSVD):
+        def build(self, return_factors="vh"):
+            return _HybridSVDDeviceMixin.build(self, return_factors=return_factors)
+
+    return PolaraB200HybridSVD, PolaraB200ScaledHybridSVD
 
 
 def dropin_sampled():
