@@ -2,6 +2,7 @@
 (``tensor.data_ptr()``), no torch op computes anything on the hot path."""
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 
 import numpy as np
@@ -97,6 +98,7 @@ class Engine:
         if st != _abi.OK:
             raise RuntimeError("pb200_ctx_create failed with status %d (an sm_90 GPU, H100, is required)" % st)
         self.h = handle
+        self.score_kernel = "tc"       # the context's default; set_score_kernel keeps this copy current
 
     def close(self):
         if getattr(self, "h", None):
@@ -146,8 +148,23 @@ class Engine:
         self._check(self.lib.pb200_ctx_sync(self.h), "sync")
 
     def set_score_kernel(self, kind):
-        kind = {"simt": 0, "tc": 1}.get(kind, kind)
-        self._check(self.lib.pb200_set_score_kernel(self.h, int(kind)), "set_score_kernel")
+        code = {"simt": 0, "tc": 1}.get(kind, kind)
+        self._check(self.lib.pb200_set_score_kernel(self.h, int(code)), "set_score_kernel")
+        self.score_kernel = ("simt", "tc")[int(code)]
+
+    @contextlib.contextmanager
+    def score_kernel_scope(self, kind):
+        """``kind`` in force inside the block (None: the current kind).  The engine is one per device and shared by every
+        model, so the kind it had before is restored after the block, also when the block raises."""
+        before = self.score_kernel
+        if kind is None or kind == before:
+            yield
+            return
+        self.set_score_kernel(kind)
+        try:
+            yield
+        finally:
+            self.set_score_kernel(before)
 
     def set_spmm_kernel(self, kind):
         kind = {"ldg": 0, "bulk": 1, "cpasync": 2, "window": 3, "window32": 4}.get(kind, kind)

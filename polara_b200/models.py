@@ -55,7 +55,7 @@ class _DeviceModelMixin:
     """State shared by the device models: engine handle and cached device buffers."""
 
     _engine = None
-    score_kernel = None          # None = engine default; 'simt' | 'tc'
+    score_kernel = None          # None = the engine's current kind; 'simt' | 'tc'
     last_timings = None
 
     @property
@@ -142,21 +142,37 @@ class _DeviceModelMixin:
             raise NotImplementedError("item projectors on an item-sharded model")
         return self._device_factor("%s_projector_right" % itemid), self._device_factor("%s_projector_left" % itemid)
 
-    def _score(self, p_dev: DeviceCSR, seen_dev, v_dev, rank, topk):
+    def _checked_test_input(self, read):
+        """``read()``, a reader of the test data that returns their shape second, between the checks the reference makes
+        around it: data integrity before, ``topk`` against the item count after (np.argpartition would raise,
+        models.py:490)."""
+        if self.verify_integrity and hasattr(self, "verify_data_integrity"):
+            self.verify_data_integrity()
+        test_input = read()
+        if self.topk > test_input[1][1]:
+            raise ValueError("topk exceeds the number of items")
+        return test_input
+
+    def _rank_lists(self, p_dev: DeviceCSR, seen_dev, v_fold, v_score, ranks):
+        """E = P v_fold once, at the padded width of the largest of the ascending ``ranks`` (the faster, unpredicated SpMM
+        variant), then the fused scoring kernel against ``v_score``: one int64 [m x topk] device tensor per rank."""
         eng = self.engine
-        if self.score_kernel is not None:
-            eng.set_score_kernel(self.score_kernel)
-        v_fold, v_dev = self._item_projector_device(v_dev)
-        e = eng.spmm(p_dev, v_fold, ell=v_fold.shape[1])    # padded width: the unpredicated SpMM variant is the faster one
+        e = eng.spmm(p_dev, v_fold, ell=round_up(ranks[-1], 32))
         seen = seen_dev if self.filter_seen else None
+        return [eng.score_topk(e, v_score, r, self.topk, seen=seen) for r in ranks]
+
+    def _score(self, p_dev: DeviceCSR, seen_dev, v_dev, rank):
+        v_fold, v_dev = self._item_projector_device(v_dev)
         shard = getattr(self, "shard", None)
-        if shard is not None:
-            # item-factor sharding: returns the lists of the user range this rank owns
-            from .dist import sharded_topk
-            ids = sharded_topk(eng, e, v_dev, rank, topk, seen, shard, p_dev.shape[0])
-            lo, hi = shard.user_range(p_dev.shape[0])
-            return ids[: hi - lo]
-        return eng.score_topk(e, v_dev, rank, topk, seen=seen)
+        if shard is None:
+            return self._rank_lists(p_dev, seen_dev, v_fold, v_dev, [rank])[0]
+        # item-factor sharding: returns the lists of the user range this rank owns
+        from .dist import sharded_topk
+        eng = self.engine
+        e = eng.spmm(p_dev, v_fold, ell=v_fold.shape[1])
+        ids = sharded_topk(eng, e, v_dev, rank, self.topk, seen_dev if self.filter_seen else None, shard, p_dev.shape[0])
+        lo, hi = shard.user_range(p_dev.shape[0])
+        return ids[: hi - lo]
 
 
 class _SVDDeviceMixin(_DeviceModelMixin):
@@ -307,62 +323,64 @@ class _SVDDeviceMixin(_DeviceModelMixin):
                 dist.broadcast(full[a:b], src=src)
         return full
 
-    stream_chunks = None     # user chunks of the pinned-CSR fast path (H2D of chunk i+1 overlaps scoring of chunk i);
+    stream_chunks = None     # user chunks of a streamed scoring call (H2D of chunk i+1 overlaps scoring of chunk i);
                              # None = stream_schedule(), an int = that many equal chunks
 
     def get_recommendations(self):
-        if self.verify_integrity and hasattr(self, "verify_data_integrity"):
-            self.verify_data_integrity()
-        eng = self.engine
+        rows, shape, is_csr, streamable = self._checked_test_input(self._test_input)
+        itemid = self.data.fields.itemid
+        rank = self.factors[itemid].shape[1]
+        with self.engine.score_kernel_scope(self.score_kernel):
+            if getattr(self, "shard", None) is None:
+                bounds = (streamable and self._stream_bounds(shape[0])) or [0, shape[0]]
+                return self._chunked_lists(rows, shape, is_csr, bounds, [rank])[0]
+            if is_csr and isinstance(rows[0], torch.Tensor):
+                return self._sharded_recommendations(*rows, shape)
+            if is_csr:
+                p_dev = self.engine.upload_csr(*rows, shape[:2])
+                seen_dev = (p_dev.indptr, p_dev.indices)
+            else:
+                p_dev, seen_dev = self._test_csr_device(rows, shape)
+            return self._score(p_dev, seen_dev, self._device_factor(itemid), rank).cpu().numpy()
+
+    def _test_input(self):
+        """``(rows, shape, is_csr, streamable)`` of a scoring call: ``rows`` is the ``(indptr, indices, values)`` of
+        ``data.test_csr`` when set, else the user-sorted ``(user, item, feedback)`` of ``_big_test_triplets()`` or else of
+        ``_get_test_data()``.  ``streamable``: a torch CSR in host memory or the triplets of a large test set."""
         fast = getattr(self.data, "test_csr", None)
         if fast is not None:
-            (indptr, indices, values), shape = fast
-            if self.topk > shape[1]:
-                raise ValueError("topk exceeds the number of items")
-            if getattr(self, "shard", None) is None and isinstance(indptr, torch.Tensor) and shape[0] >= 4 * 65536:
-                return self._streamed_recommendations(indptr, indices, values, shape)
-            if getattr(self, "shard", None) is not None and isinstance(indptr, torch.Tensor):
-                return self._sharded_recommendations(indptr, indices, values, shape)
-            t0 = time.perf_counter()
-            p_dev = eng.upload_csr(indptr, indices, values, shape[:2])
-            seen_dev = (p_dev.indptr, p_dev.indices)
-        else:
-            # the route a Polara user takes: triplets of test_to_coo (sorted by user) -> device ingest -> scoring
-            big = self._big_test_triplets()
-            if big is not None:
-                test_data, shape = big
-                if self.topk > shape[1]:
-                    raise ValueError("topk exceeds the number of items")
-                return self._streamed_recommendations(None, None, None, shape, triplets=test_data)
-            test_data, shape, _ = self._get_test_data()
-            if self.topk > shape[1]:
-                raise ValueError("topk exceeds the number of items")   # np.argpartition would raise, models.py:490
-            t0 = time.perf_counter()
-            p_dev, seen_dev = self._test_csr_device(test_data, shape)
-        v_dev = self._device_factor(self.data.fields.itemid)
-        if getattr(self, "profile_phases", False):
-            torch.cuda.synchronize()
-        t1 = time.perf_counter()
-        ids = self._score(p_dev, seen_dev, v_dev, self.factors[self.data.fields.itemid].shape[1], self.topk)
-        if getattr(self, "profile_phases", False):
-            torch.cuda.synchronize()
-        t2 = time.perf_counter()
-        out = ids.cpu().numpy()
-        self.last_score_timings = dict(h2d_s=t1 - t0, score_s=t2 - t1, d2h_s=time.perf_counter() - t2)
-        return out
+            rows, shape = fast
+            return rows, shape, True, isinstance(rows[0], torch.Tensor)
+        big = self._big_test_triplets()
+        if big is not None:
+            return big[0], big[1], False, True
+        test_data, shape, _ = self._get_test_data()
+        return test_data, shape, False, False
+
+    def _stream_bounds(self, m):
+        """User-chunk bounds of a streamed scoring call over ``m`` test users, or None when there are too few to stream.
+        The bounds fix the last bits of the result: SpMM windows are counted from each launch's first nnz (DESIGN.md
+        section 4), so E, and with it a near-tied list, depends on where the rows are cut."""
+        if m < 4 * 65536:
+            return None
+        if self.stream_chunks is None:
+            sms = torch.cuda.get_device_properties(self.engine.device).multi_processor_count
+            return stream_schedule(m, sms * 128)
+        n_chunks = max(1, int(self.stream_chunks))
+        return [m * c // n_chunks for c in range(n_chunks + 1)]
 
     def _big_test_triplets(self):
-        """Large test sets skip the host-side passes of ``_get_test_data`` (models.py:227-257: np.diff over all triplets
-        for the sortedness assert and the gap test -- four passes over 1e8 int64 cost more than the whole device path).
-        The same facts are established differently: the ingest kernel checks the order of every chunk on the device (and
-        sorts if it has to), and users that start at 0 and end at n_test_users - 1 leave no room for a gap because
-        ``get_test_shape`` counts the distinct test users (data.py:865-884).  Anything else returns None and takes the
-        reference's path."""
+        """Large test sets (those that are streamed, ``_stream_bounds``) skip the host-side passes of ``_get_test_data``
+        (models.py:227-257: np.diff over all triplets for the sortedness assert and the gap test -- four passes over 1e8
+        int64 cost more than the whole device path).  The same facts are established differently: the ingest kernel checks
+        the order of every chunk on the device (and sorts if it has to), and users that start at 0 and end at
+        n_test_users - 1 leave no room for a gap because ``get_test_shape`` counts the distinct test users
+        (data.py:865-884).  Anything else returns None and takes the reference's path."""
         if getattr(self, "shard", None) is not None:
             return None
         data = self.data
         shape = data.get_test_shape(tensor_mode=False)
-        if shape[0] < 4 * 65536:
+        if self._stream_bounds(shape[0]) is None:
             return None
         threshold = None if data.warm_start else self.feedback_threshold
         user, item, fdbk = data.test_to_coo(tensor_mode=False, feedback_threshold=threshold)
@@ -381,8 +399,6 @@ class _SVDDeviceMixin(_DeviceModelMixin):
         rank_r = self.factors[self.data.fields.itemid].shape[1]
         v_dev = self._device_factor(self.data.fields.itemid)
         self._item_projector_device(v_dev)                    # raises for a model that carries item projectors
-        if self.score_kernel is not None:
-            eng.set_score_kernel(self.score_kernel)
         indptr64 = indptr if indptr.dtype == torch.int64 else indptr.to(torch.int64)
         world = shard.world
         chunk_u = shard.user_chunk(m)
@@ -428,57 +444,71 @@ class _SVDDeviceMixin(_DeviceModelMixin):
             self.last_score_timings = dict(zip(("h2d_s", "assemble_s", "score_s", "d2h_s"), np.diff(tp).round(4)))
         return out
 
-    def _streamed_recommendations(self, indptr, indices, values, shape, triplets=None):
-        """Host test data -> recommendations in user chunks: the H2D copy of chunk i+1 (side stream) overlaps ingest +
-        SpMM + fused scoring of chunk i (context stream); results go back into one pinned buffer on a third stream.
-        Two sources: a pinned host CSR (``data.test_csr``) or, with ``triplets``, the user-sorted
-        ``(user, item, feedback)`` arrays of ``test_to_coo`` -- what a Polara data model hands over -- which are
-        converted to CSR on the device chunk by chunk (pb200_coo_to_csr)."""
+    def _chunked_lists(self, rows, shape, is_csr, bounds, ranks):
+        """Host test rows -> one int64 [m x topk] array of lists per rank of the ascending ``ranks``, scored in the user
+        chunks ``bounds``: the H2D copy of chunk i+1 (side stream) overlaps ingest + SpMM + fused scoring of chunk i
+        (context stream); the lists go back into one pinned buffer on a third stream.  One chunk has nothing to overlap and
+        runs in order on the context stream (unless ``profile_phases`` wants its events).  ``rows``: a host CSR
+        (``is_csr``; numpy or torch) or the user-sorted ``(user, item, feedback)`` arrays of ``test_to_coo``, converted
+        to CSR on the device chunk by chunk (pb200_coo_to_csr)."""
         t_entry = time.perf_counter()
         eng = self.engine
         m, n_items = shape[0], shape[1]
-        rank = self.factors[self.data.fields.itemid].shape[1]
-        v_dev = self._device_factor(self.data.fields.itemid)
-        v_fold, v_score = self._item_projector_device(v_dev)
-        if self.score_kernel is not None:
-            eng.set_score_kernel(self.score_kernel)
-        if self.stream_chunks is None:
-            sms = torch.cuda.get_device_properties(eng.device).multi_processor_count
-            bounds = stream_schedule(m, sms * 128)
-        else:
-            n_chunks = max(1, int(self.stream_chunks))
-            bounds = [m * c // n_chunks for c in range(n_chunks + 1)]
+        v_fold, v_score = self._item_projector_device(self._device_factor(self.data.fields.itemid))
         n_chunks = len(bounds) - 1
-        # fresh pinned result buffer: torch's caching host allocator re-uses the block once the previous result is
-        # garbage-collected, so steady-state calls pay neither cudaHostAlloc nor page faults, and results never alias
-        out = torch.empty((m, self.topk), dtype=torch.int64, pin_memory=True)
-        main = torch.cuda.current_stream(eng.device)
-        side = self.__dict__.setdefault("_copy_stream", torch.cuda.Stream(device=eng.device))
-        back = self.__dict__.setdefault("_result_stream", torch.cuda.Stream(device=eng.device))
         prof = [] if getattr(self, "profile_phases", False) else None
-        if triplets is None:
+        if is_csr:
+            indptr, indices, values = (x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
+                                       for x in rows)
             indptr64 = indptr if indptr.dtype == torch.int64 else indptr.to(torch.int64)
-            cuts = [int(indptr64[b]) for b in bounds]
             host = (indices, values)
         else:
-            user, item, fdbk = (np.asarray(x) for x in triplets)
+            user, item, fdbk = (np.asarray(x) for x in rows)
+            host = tuple(torch.from_numpy(x) for x in (_as_index_array(user), _as_index_array(item), _as_value_array(fdbk)))
+        if n_chunks == 1:
+            cuts = [0, None]                               # nothing to cut: the arrays go up as they are
+        elif is_csr:
+            cuts = [int(indptr64[b]) for b in bounds]
+        else:
             cuts = [int(c) for c in np.searchsorted(user, np.asarray(bounds))]
             # the chunks are cut on the assumption that the triplets are sorted by user (the reference asserts it,
             # models.py:246): inside a chunk the ingest kernel verifies it, across the cuts it is verified here
             for bnd, cut in zip(bounds[1:-1], cuts[1:-1]):
                 if (cut > 0 and user[cut - 1] >= bnd) or (cut < len(user) and user[cut] < bnd):
                     raise AssertionError("calculations assume testset is sorted by users!")
-            host = tuple(torch.from_numpy(x) for x in (_as_index_array(user), _as_index_array(item), _as_value_array(fdbk)))
 
-        def upload(c):
+        def upload(c):                                     # chunk c -> the device, on the current stream
             a, b = bounds[c], bounds[c + 1]
             lo, hi = cuts[c], cuts[c + 1]
+            head = (indptr64[a:b + 1].to(eng.device, non_blocking=True),) if is_csr else ()
+            return head + tuple(t[lo:hi].to(eng.device, non_blocking=True) for t in host), a, b, lo
+
+        def ingest(dev, a, b, lo):                         # -> the chunk's P and seen pattern
+            if is_csr:
+                ip, ix, vl = dev
+                if lo:
+                    eng.shift_i64(ip, -lo)                 # re-base the row pointers of the chunk
+                p_dev = DeviceCSR(ip, ix if ix.dtype == torch.int32 else ix.to(torch.int32),
+                                  vl if vl.dtype == torch.float32 else vl.to(torch.float32), (b - a, n_items))
+                return p_dev, (p_dev.indptr, p_dev.indices)
+            u_d, i_d, f_d = dev
+            if a:
+                eng.shift_i64(u_d, -a)                     # users of the chunk count from 0
+            return self._test_csr_device(None, (b - a, n_items), stream_arrays=(u_d, i_d, f_d, None), sorted_users=True)
+
+        if n_chunks == 1 and prof is None:
+            return [ids.cpu().numpy() for ids in self._rank_lists(*ingest(*upload(0)), v_fold, v_score, ranks)]
+
+        # fresh pinned result buffer: torch's caching host allocator re-uses the block once the previous result is
+        # garbage-collected, so steady-state calls pay neither cudaHostAlloc nor page faults, and results never alias
+        out = torch.empty((len(ranks), m, self.topk), dtype=torch.int64, pin_memory=True)
+        main = torch.cuda.current_stream(eng.device)
+        side = self.__dict__.setdefault("_copy_stream", torch.cuda.Stream(device=eng.device))
+        back = self.__dict__.setdefault("_result_stream", torch.cuda.Stream(device=eng.device))
+
+        def upload_aside(c):
             with torch.cuda.stream(side):
-                if triplets is None:
-                    dev = (indptr64[a:b + 1].to(eng.device, non_blocking=True),) + \
-                        tuple(t[lo:hi].to(eng.device, non_blocking=True) for t in host)
-                else:
-                    dev = tuple(t[lo:hi].to(eng.device, non_blocking=True) for t in host)
+                dev, a, b, lo = upload(c)
                 ev = torch.cuda.Event(enable_timing=prof is not None)
                 ev.record(side)
             return (dev, ev, a, b, lo)
@@ -493,42 +523,32 @@ class _SVDDeviceMixin(_DeviceModelMixin):
         side.wait_stream(main)
         if prof is not None:
             ev_start = mark(main)
-        nxt = upload(0)
+        nxt = upload_aside(0)
         keep = []
         for c in range(n_chunks):
             dev, ev, a, b, lo = nxt
             if c + 1 < n_chunks:
-                nxt = upload(c + 1)
+                nxt = upload_aside(c + 1)
             main.wait_event(ev)
             if prof is not None:
                 prof.append(["chunk%d" % c, ev, mark(main), None, None, time.perf_counter() - t_host0])
             for t in dev:
                 t.record_stream(main)                      # allocated on the side stream, consumed on the main one
-            if triplets is None:
-                ip, ix, vl = dev
-                eng.shift_i64(ip, -lo)                     # re-base the row pointers of the chunk
-                p_dev = DeviceCSR(ip, ix if ix.dtype == torch.int32 else ix.to(torch.int32),
-                                  vl if vl.dtype == torch.float32 else vl.to(torch.float32), (b - a, n_items))
-                seen = (p_dev.indptr, p_dev.indices)
-            else:
-                u_d, i_d, f_d = dev
-                eng.shift_i64(u_d, -a)                     # users of the chunk count from 0
-                p_dev, seen = self._test_csr_device(None, (b - a, n_items), stream_arrays=(u_d, i_d, f_d, None),
-                                                    sorted_users=True)
-            e = eng.spmm(p_dev, v_fold, ell=v_fold.shape[1])
-            ids = eng.score_topk(e, v_score, rank, self.topk, seen=seen if self.filter_seen else None)
+            p_dev, seen = ingest(dev, a, b, lo)
+            ids = self._rank_lists(p_dev, seen, v_fold, v_score, ranks)
             if prof is not None:
                 prof[-1][3] = mark(main)
             scored = torch.cuda.Event()
             scored.record(main)
             with torch.cuda.stream(back):                  # results leave on their own stream / copy engine
                 back.wait_event(scored)
-                out[a:b].copy_(ids, non_blocking=True)
+                for j, t in enumerate(ids):
+                    out[j, a:b].copy_(t, non_blocking=True)
                 done = torch.cuda.Event(enable_timing=prof is not None)
                 done.record(back)
             if prof is not None:
                 prof[-1][4] = done
-            keep.append((p_dev, seen, e, ids))
+            keep.append((p_dev, seen, ids))
         main.synchronize()
         back.synchronize()
         if prof is not None:
@@ -537,7 +557,7 @@ class _SVDDeviceMixin(_DeviceModelMixin):
                 "host_total_ms": (time.perf_counter() - t_host0) * 1e3, "setup_ms": (t_host0 - t_entry) * 1e3,
                 "chunks": [[name, ev_start.elapsed_time(up), ev_start.elapsed_time(c0), ev_start.elapsed_time(c1),
                             ev_start.elapsed_time(d1), host_t * 1e3] for name, up, c0, c1, d1, host_t in prof]}
-        return out.numpy()
+        return list(out.numpy())
 
     # ---- sampled evaluation (RandomSampleEvaluationSVDMixin, models.py:1095-1183) ---------------------------------------
     def sampled_recommendations(self, holdout_items, unseen_items=None, test_data=None, shape=None, n_unseen=None, seed=None,
@@ -583,24 +603,12 @@ class _SVDDeviceMixin(_DeviceModelMixin):
         rank, made once: one test-data ingest, one SpMM at the largest rank (through the right item projector for a model
         that carries HybridSVD projectors), then the fused scoring kernel once per rank on the leading columns of the
         same embeddings, honouring ``filter_seen`` and ``score_kernel``.  Returns ``{rank: int64 [n_test_users x topk]}``.
-        The test triplets are read as ``get_recommendations`` reads them (``_big_test_triplets`` for large test sets,
-        else ``_get_test_data``).  Same note on the embeddings as ``sampled_rank_sweep``."""
+        The test data are read as ``get_recommendations`` reads them (``_test_input``) and scored in one chunk.  Same
+        note on the embeddings as ``sampled_rank_sweep``."""
         ranks = self._sweep_ranks(ranks)
-        if self.verify_integrity and hasattr(self, "verify_data_integrity"):
-            self.verify_data_integrity()
-        eng = self.engine
-        big = self._big_test_triplets()
-        test_data, shape = big if big is not None else self._get_test_data()[:2]
-        if self.topk > shape[1]:
-            raise ValueError("topk exceeds the number of items")
-        p_dev, seen_dev = self._test_csr_device(test_data, shape, sorted_users=big is not None)
-        v_dev = self._device_factor(self.data.fields.itemid)
-        if self.score_kernel is not None:
-            eng.set_score_kernel(self.score_kernel)
-        v_fold, v_score = self._item_projector_device(v_dev)
-        e = eng.spmm(p_dev, v_fold, ell=min(v_fold.shape[1], round_up(ranks[-1], 32)))
-        seen = seen_dev if self.filter_seen else None
-        return {r: eng.score_topk(e, v_score, r, self.topk, seen=seen).cpu().numpy() for r in ranks}
+        rows, shape, is_csr, _ = self._checked_test_input(self._test_input)
+        with self.engine.score_kernel_scope(self.score_kernel):
+            return dict(zip(ranks, self._chunked_lists(rows, shape, is_csr, [0, shape[0]], ranks)))
 
     def _sweep_ranks(self, ranks):
         """the distinct ranks of a sweep, ascending; each must be a truncation of the current factors."""
@@ -1122,21 +1130,15 @@ class _CoffeeDeviceMixin(_DeviceModelMixin):
         self.core_norm_trace = trace
 
     def get_recommendations(self):
-        if self.verify_integrity and hasattr(self, "verify_data_integrity"):
-            self.verify_data_integrity()
-        eng = self.engine
+        (user, item, fdbk_idx), shape, _ = self._checked_test_input(self._get_test_data)
         f = self.data.fields
-        test_data, shape, _ = self._get_test_data()
-        user, item, fdbk_idx = test_data
         w = self.factors[f.feedback]
         # E[u,:] = sum_{(i,f) in u} (w[f,:] . wt_flat) v[i,:]   (SURVEY.md §8a row A9)
         c = np.asarray(w) @ flatten_weights(w, self.flattener)
         weights = c[np.asarray(fdbk_idx, dtype=np.int64)].astype(np.float32)
-        if self.topk > shape[1]:
-            raise ValueError("topk exceeds the number of items")
         p_dev, seen_dev = self._test_csr_device((user, item, None), shape, values=weights)
-        v_dev = self._device_factor(f.itemid)
-        ids = self._score(p_dev, seen_dev, v_dev, self.factors[f.itemid].shape[1], self.topk)
+        with self.engine.score_kernel_scope(self.score_kernel):
+            ids = self._score(p_dev, seen_dev, self._device_factor(f.itemid), self.factors[f.itemid].shape[1])
         return ids.cpu().numpy()
 
 
@@ -1257,11 +1259,7 @@ class _CooccurrenceDeviceMixin(_DeviceModelMixin):
             print("{} training time: {:.3f}s".format(self.method, t1 - t0))
 
     def get_recommendations(self):
-        if self.verify_integrity and hasattr(self, "verify_data_integrity"):
-            self.verify_data_integrity()
-        test_data, shape, _ = self._get_test_data()
-        if self.topk > shape[1]:
-            raise ValueError("topk exceeds the number of items")
+        test_data, shape, _ = self._checked_test_input(self._get_test_data)
         nnz, dense, sparse = self.i2i_lists(test_data, shape)
         out = np.empty((shape[0], self.topk), dtype=np.int64)
         for a, b, is_dense in cooc_chunk_modes(nnz, shape[1], self.topk, self._memory_hard_limit(), self.dense_output):
