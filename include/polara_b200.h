@@ -360,6 +360,29 @@ int pb200_i2i_topk(pb200_ctx* ctx, const double* S, int64_t lds, int64_t n, int6
                    const int32_t* seen_indices, int implicit, int k, int64_t* out_nnz, int64_t* out_dense,
                    int64_t* out_sparse, double* out_scores);
 
+/* Sparse storage of the item-to-item matrix, for catalogues whose dense S does not fit.
+ * pb200_cooc_build_csr: the S of pb200_cooc_build as an fp64 CSR [n x n]: rows with ascending column ids, no diagonal
+ *   and no entry that sums to exactly 0 (eliminate_zeros); every stored entry has the bits of the dense build's entry.
+ *   `a` is the plain training CSR (one panel), `at` the plain CSR of A^T.  Two calls with the same a, at and implicit:
+ *     fill == 0  counts the rows: indptr (device int64 [n+1]) gets the row offsets, *nnz (HOST) the total, so the
+ *                caller can check the memory before allocating the rows;
+ *     fill != 0  writes the rows (device int32 / fp64 [*nnz]) at those offsets; *nnz is the count of the first call
+ *                (0: nothing to write, indices / values may be NULL).
+ *   acc_rows: at most this many rows of n doubles of global scratch for the item rows whose work exceeds a
+ *   shared-memory table (at least 1; each CTA of that path owns one; only as many as there are such rows are taken). */
+int pb200_cooc_build_csr(pb200_ctx* ctx, const pb200_csr_view* a, const pb200_csr_view* at, int implicit, int acc_rows,
+                         int fill, int64_t* indptr, int32_t* indices, double* values, int64_t* nnz);
+/* pb200_i2i_topk_csr: pb200_i2i_topk with S given as an fp64 CSR [n x n] (s_indptr int64 [n+1], s_indices int32 sorted,
+ *   s_values fp64), with the same outputs, bit-equal to pb200_i2i_topk on the dense form of the same S.  acc_rows: at
+ *   most this many rows of n doubles of global scratch for the users whose work (the nonzeros of their S rows) exceeds
+ *   a shared-memory table (at least 1; each warp of that path owns one; only as many as there are such users are
+ *   taken).  Scratch besides: m * 2k * 16 + 24 m bytes.  No [m x n] block is formed. */
+int pb200_i2i_topk_csr(pb200_ctx* ctx, int64_t n, const int64_t* s_indptr, const int32_t* s_indices,
+                       const double* s_values, int64_t m, const int64_t* p_indptr, const int32_t* p_indices,
+                       const float* p_values, const int64_t* seen_indptr, const int32_t* seen_indices, int implicit,
+                       int k, int acc_rows, int64_t* out_nnz, int64_t* out_dense, int64_t* out_sparse,
+                       double* out_scores);
+
 /* res[i0,:,:] += val * U[i1,:] (x) W[i2,:] over all nnz of a 3-way COO tensor sorted
  * and grouped by mode-0 index (CSR-like: seg_ptr int64 [n0+1], i1/i2 int32 [nnz]);
  * out [n0 x ru*rw] row-major (ld = ldo).  Replaces dttm_seq/dttm_par,

@@ -73,6 +73,10 @@ _SIGNATURES = {
     "pb200_sampler_stats": ([ptr, C.POINTER(C.c_uint64)], C.c_int),
     "pb200_cooc_build": ([ptr, C.POINTER(CsrView), C.POINTER(CsrView), C.c_int, ptr, i64], C.c_int),
     "pb200_i2i_topk": ([ptr, ptr, i64, i64, i64, ptr, ptr, ptr, ptr, ptr, C.c_int, C.c_int, ptr, ptr, ptr, ptr], C.c_int),
+    "pb200_cooc_build_csr": ([ptr, C.POINTER(CsrView), C.POINTER(CsrView), C.c_int, C.c_int, C.c_int, ptr, ptr, ptr,
+                              C.POINTER(i64)], C.c_int),
+    "pb200_i2i_topk_csr": ([ptr, i64, ptr, ptr, ptr, i64, ptr, ptr, ptr, ptr, ptr, C.c_int, C.c_int, C.c_int, ptr, ptr,
+                            ptr, ptr], C.c_int),
     "pb200_score_dense": ([ptr, ptr, i64, ptr, i64, i64, i64, C.c_int, ptr, i64], C.c_int),
     "pb200_ttm": ([ptr, i64, i64, ptr, ptr, ptr, ptr, ptr, C.c_int, i64, ptr, C.c_int, i64, ptr, i64], C.c_int),
     "pb200_ttm_reduce": ([ptr, C.c_int, i64, ptr, ptr, ptr, ptr, ptr, C.c_int, i64, ptr, C.c_int, i64, ptr, i64],

@@ -33,7 +33,8 @@ def round_up(x, m):
 
 
 class DeviceCSR:
-    """CSR matrix resident in HBM: indptr int64, indices int32, values float32.  ``n_panels > 1``: panel-major storage
+    """CSR matrix resident in HBM: indptr int64, indices int32, values float32 (float64 for the item-to-item matrix of
+    ``Engine.cooc_build_csr``, which only ``Engine.i2i_topk_csr`` reads).  ``n_panels > 1``: panel-major storage
     (``pb200_csr_block_columns``): indptr has n_panels * n_rows + 1 entries, ``panel_ptr`` is the host array of panel
     offsets."""
 
@@ -50,13 +51,16 @@ class DeviceCSR:
         return int(self.indices.shape[0])
 
     def view(self):
-        """the ``pb200_csr_view`` struct for the C-ABI (holds raw pointers: keep ``self`` alive while it is used)."""
+        """the ``pb200_csr_view`` struct for the C-ABI (holds raw pointers: keep ``self`` alive while it is used).  Its
+        values are float32: every entry point that takes a view reads them so."""
+        if self.values.dtype != torch.float32:
+            raise TypeError("a pb200_csr_view holds float32 values, got %s" % self.values.dtype)
         return _abi.CsrView(self.shape[0], self.shape[1], self.nnz, self.indptr.data_ptr(), self.indices.data_ptr(),
                             self.values.data_ptr(), self.n_panels, self.panel_cols,
                             C.cast(self.panel_ptr, C.c_void_p) if self.panel_ptr is not None else None)
 
     def nbytes(self):
-        return self.indptr.numel() * 8 + self.indices.numel() * 4 + self.values.numel() * 4
+        return self.indptr.numel() * 8 + self.indices.numel() * 4 + self.values.numel() * self.values.element_size()
 
 
 class _StreamFollowingLib:
@@ -317,13 +321,13 @@ class Engine:
         t = DeviceCSR(self.empty((a.shape[1] + 1,), torch.int64), self.empty((a.nnz,), torch.int32),
                       self.empty((a.nnz,), torch.float32), (a.shape[1], a.shape[0]))
         st = self.lib.pb200_csr_transpose(self.h, a.shape[0], a.shape[1], a.nnz, _p(a.indptr), _p(a.indices),
-                                          _p(a.values), _p(t.indptr), _p(t.indices), _p(t.values))
+                                          _p(a.values, _F32), _p(t.indptr), _p(t.indices), _p(t.values))
         self._check(st, "csr_transpose")
         return t
 
     def rescale(self, a: DeviceCSR, row_scaling, col_scaling):
         st = self.lib.pb200_rescale(self.h, a.shape[0], a.shape[1], a.nnz, _p(a.indptr), _p(a.indices),
-                                    _p(a.values), float(row_scaling), float(col_scaling))
+                                    _p(a.values, _F32), float(row_scaling), float(col_scaling))
         self._check(st, "rescale")
 
     def rsvd(self, a: DeviceCSR, at: DeviceCSR, rank, ell, max_iters=8, tol=1e-6, seed=1, want_u=False, vec_tol=0.0,
@@ -512,7 +516,7 @@ class Engine:
         n_panels = -(-n // panel_cols)
         scratch = (0 if at is not None else a.nbytes() + 8 * n) + (a.nbytes() + 8 * n_panels * m if n_panels > 1 else 0) \
             + 32 * n
-        cooc_memory_check(n, scratch, torch.cuda.mem_get_info(self.device)[0])
+        cooc_memory_check(n, scratch, self.free_bytes())
         if at is None:
             at = self.transpose(a)
         a_blk = self.block_columns(a, panel_cols)
@@ -522,6 +526,85 @@ class Engine:
         st = self.lib.pb200_cooc_build(self.h, C.byref(va), C.byref(vt), int(bool(implicit)), _p(s, _F64), lds)
         self._check(st, "cooc_build")
         return s
+
+    def free_bytes(self):
+        """free device memory in bytes: what the item-to-item builds check their allocations against."""
+        return torch.cuda.mem_get_info(self.device)[0]
+
+    # global scratch of the sparse item-to-item kernels: rows of n_items doubles for the item rows (build) and the users
+    # (scoring) too long for a shared-memory table; the row count is capped by a byte budget and a row limit.  Scoring
+    # gets the larger budget: each of its rows is one warp, and those warps are what keeps the HBM busy on long users.
+    COOC_CSR_ACC_BYTES, COOC_CSR_ACC_ROWS = 256 << 20, 512        # build: one CTA of 256 threads per row
+    I2I_CSR_ACC_BYTES, I2I_CSR_ACC_ROWS = 2 << 30, 2048           # scoring: one warp per row
+
+    @staticmethod
+    def _csr_acc_rows(n_items, budget, limit):
+        return int(max(1, min(limit, budget // (8 * max(int(n_items), 1)))))
+
+    def cooc_build_csr(self, a: DeviceCSR, implicit=False, at=None):
+        """the item-to-item matrix of ``cooc_build`` as a DeviceCSR with float64 values (pb200_cooc_build_csr): sorted
+        column ids, no diagonal, no stored zero, every entry bit-equal to the dense build's.  Two passes: the first counts
+        the entries; ``cooc_csr_memory_check`` then refuses with MemoryError, before the rows are allocated, when they
+        and the second pass's scratch do not fit the device's free memory.  The same check runs before the first pass
+        on its scratch alone."""
+        m, n = a.shape
+        if a.n_panels > 1:
+            raise ValueError("cooc_build_csr: `a` must be a plain CSR")
+        rows = self._csr_acc_rows(n, self.COOC_CSR_ACC_BYTES, self.COOC_CSR_ACC_ROWS)
+        scratch = rows * n * 8 + csr_sort_scratch_bytes(n)     # global rows (at most), schedule and sort buffers
+        cooc_csr_memory_check(0, n, scratch + (0 if at is not None else a.nbytes() + 8 * n), self.free_bytes())
+        if at is None:
+            at = self.transpose(a)
+        indptr = self.empty((n + 1,), torch.int64)
+        total = C.c_int64(0)
+        va, vt = a.view(), at.view()
+        st = self.lib.pb200_cooc_build_csr(self.h, C.byref(va), C.byref(vt), int(bool(implicit)), rows, 0,
+                                           _p(indptr, _I64), None, None, C.byref(total))
+        self._check(st, "cooc_build_csr")
+        nnz = int(total.value)
+        try:
+            # the first pass's scratch goes back to the device once its frees have run; indptr is already allocated:
+            # it counts in the need and in what is free
+            self.sync()
+            cooc_csr_memory_check(nnz, n, scratch, self.free_bytes() + indptr.numel() * 8)
+        except MemoryError:
+            del indptr, at, va, vt                         # nothing of the build outlives the refusal
+            raise
+        indices = self.empty((nnz,), torch.int32)
+        values = self.empty((nnz,), torch.float64)
+        # with nnz == 0 both tensors are empty and their pointers NULL: the fill call then only returns
+        st = self.lib.pb200_cooc_build_csr(self.h, C.byref(va), C.byref(vt), int(bool(implicit)), rows, 1,
+                                           _p(indptr, _I64), _p(indices, _I32), _p(values, _F64), C.byref(total))
+        self._check(st, "cooc_build_csr")
+        return DeviceCSR(indptr, indices, values, (n, n))
+
+    def i2i_topk_csr(self, s_csr: DeviceCSR, p: DeviceCSR, k, seen=None, implicit=False, want_scores=False):
+        """``i2i_topk`` with S a float64 DeviceCSR (``cooc_build_csr``, or a caller's item x item matrix) through
+        pb200_i2i_topk_csr: the same outputs, bit-equal to ``i2i_topk`` on the dense form of the same S.  Refuses with
+        MemoryError, before allocating anything, when the outputs, the lists and one global row do not fit the device's
+        free memory; the global rows take at most half of what is left (``I2I_CSR_ACC_BYTES`` at most)."""
+        n = s_csr.shape[1]
+        if s_csr.shape[0] != n or p.shape[1] != n:
+            raise ValueError("i2i_topk_csr: S must be [n_items x n_items] and P [m x n_items]")
+        m = p.shape[0]
+        fixed = m * (8 + 8 * k * (3 if want_scores else 2)) + m * 2 * k * 16 + csr_sort_scratch_bytes(m)
+        free = self.free_bytes()
+        if fixed + 8 * n > free:
+            raise MemoryError("item-to-item scoring: %d test users at k = %d need %d bytes of outputs and scratch plus "
+                              "%d for one accumulator row, but only %d bytes of device memory are free"
+                              % (m, k, fixed, 8 * n, free))
+        rows = self._csr_acc_rows(n, min(self.I2I_CSR_ACC_BYTES, (free - fixed) // 2), self.I2I_CSR_ACC_ROWS)
+        nnz = self.empty((m,), torch.int64)
+        dense = self.empty((m, k), torch.int64)
+        sparse = self.empty((m, k), torch.int64)
+        scores = self.empty((m, k), torch.float64) if want_scores else None
+        sp, si = (seen if seen is not None else (None, None))
+        st = self.lib.pb200_i2i_topk_csr(self.h, n, _p(s_csr.indptr, _I64), _p(s_csr.indices, _I32),
+                                         _p(s_csr.values, _F64), m, _p(p.indptr, _I64), _p(p.indices, _I32),
+                                         _p(p.values, _F32), _p(sp, _I64), _p(si, _I32), int(bool(implicit)), int(k),
+                                         rows, _p(nnz), _p(dense), _p(sparse), _p(scores))
+        self._check(st, "i2i_topk_csr")
+        return (nnz, dense, sparse, scores) if want_scores else (nnz, dense, sparse)
 
     def i2i_topk(self, s, n_items, p: DeviceCSR, k, seen=None, implicit=False, want_scores=False):
         """per test user the nonzero count of ``P S`` and its top-k lists under the dense and the sparse chunk rule
@@ -600,13 +683,37 @@ def cooc_lds(n_items):
 
 def cooc_memory_check(n_items, scratch_bytes, free_bytes):
     """Raises MemoryError when the dense fp64 item-to-item matrix of ``n_items`` items plus ``scratch_bytes`` exceeds
-    ``free_bytes`` (the device's free memory); storing S sparsely for larger catalogues is not implemented."""
+    ``free_bytes`` (the device's free memory); larger catalogues take the sparse form (``cooc_build_csr``)."""
     need_s = int(n_items) * cooc_lds(n_items) * 8
     need = need_s + int(scratch_bytes)
     if need > int(free_bytes):
         raise MemoryError("item-to-item model: the dense item x item matrix of %d items takes %d bytes (plus %d bytes of "
                           "scratch, %d in all), but only %d bytes of device memory are free"
                           % (int(n_items), need_s, int(scratch_bytes), need, int(free_bytes)))
+    return need
+
+
+def csr_sort_scratch_bytes(count):
+    """scratch of the sparse item-to-item kernels' longest-first schedule over ``count`` rows or users: work, order and
+    the radix sort's key and value buffers (about 48 bytes each), with a fixed margin for the sort's and scan's
+    temporary storage."""
+    return 64 * int(count) + (16 << 20)
+
+
+def cooc_csr_bytes(nnz, n_items):
+    """bytes of the item-to-item matrix as an fp64 CSR: int64 row offsets, int32 column ids, fp64 values."""
+    return 8 * (int(n_items) + 1) + 12 * int(nnz)
+
+
+def cooc_csr_memory_check(nnz, n_items, scratch_bytes, free_bytes):
+    """Raises MemoryError when the sparse fp64 item-to-item matrix of ``n_items`` items with ``nnz`` stored entries plus
+    ``scratch_bytes`` exceeds ``free_bytes`` (the device's free memory)."""
+    need_s = cooc_csr_bytes(nnz, n_items)
+    need = need_s + int(scratch_bytes)
+    if need > int(free_bytes):
+        raise MemoryError("item-to-item model: the sparse item x item matrix of %d items with %d stored entries takes %d "
+                          "bytes (plus %d bytes of scratch, %d in all), but only %d bytes of device memory are free"
+                          % (int(n_items), int(nnz), need_s, int(scratch_bytes), need, int(free_bytes)))
     return need
 
 

@@ -36,8 +36,11 @@ class ArrayData:
 
     def __init__(self, train_idx, train_val, train_shape, test_user=None, test_item=None, test_fdbk=None,
                  test_shape=None, holdout=None, warm_start=True, fields=("userid", "itemid", "rating"),
-                 n_feedback=None, holdout_size=3):
+                 n_feedback=None, holdout_size=3, item_relations=None):
         self.fields = Fields(*fields)
+        # item x item side relations (SimilarityDataModel.item_relations, hybrid/data.py:25-28), in the item index of
+        # the training data; read by B200SimilarityAggregation
+        self.item_relations = item_relations
         self._train = (np.asarray(train_idx), np.asarray(train_val), tuple(int(s) for s in train_shape))
         self._test_coo = None if test_user is None else (np.asarray(test_user), np.asarray(test_item),
                                                          np.asarray(test_fdbk))

@@ -23,7 +23,8 @@ from . import host
 from .engine import DeviceCSR, get_engine, round_up
 
 __all__ = ["B200SVDModel", "B200ScaledSVD", "B200HybridSVD", "B200ScaledHybridSVD", "B200CoffeeModel",
-           "B200CooccurrenceModel", "dropin", "dropin_hybrid", "dropin_i2i", "default_ell"]
+           "B200CooccurrenceModel", "B200SimilarityAggregation", "dropin", "dropin_hybrid", "dropin_i2i",
+           "dropin_similarity", "default_ell"]
 
 
 def default_ell(rank, oversample=None):
@@ -1236,8 +1237,15 @@ def cooc_chunk_modes(nnz_u, n_items, topk, memory_hard_limit, dense_output=False
 
 class _CooccurrenceDeviceMixin(_DeviceModelMixin):
     """Device implementation of CooccurrenceModel.build / get_recommendations (models.py:693-725, 391-405): S = A^T A
-    stays on the device as a dense fp64 matrix; scoring computes every test user's ``P S`` row once and returns its list
-    under the rule the reference's chunk of that user applies (``cooc_chunk_modes``)."""
+    stays on the device, as a dense fp64 matrix or as an fp64 CSR (``storage``); scoring computes every test user's
+    ``P S`` row once and returns its list under the rule the reference's chunk of that user applies
+    (``cooc_chunk_modes``).  Both forms give the same bits.
+
+    ``storage``: ``"auto"`` builds S dense wherever it fits the device and sparse only where the dense build would
+    refuse with MemoryError; ``"dense"`` always dense (and that refusal); ``"sparse"`` always the CSR."""
+
+    storage = "auto"
+    i2i_storage = None           # the form the last build took: "dense" | "sparse"
 
     def _memory_hard_limit(self):
         return host.DEFAULTS["memory_hard_limit"]
@@ -1245,11 +1253,22 @@ class _CooccurrenceDeviceMixin(_DeviceModelMixin):
     def build(self):
         data = self.data
         idx, val, shape = data.to_coo(tensor_mode=False, feedback_threshold=self.feedback_threshold)
+        if self.storage not in ("auto", "dense", "sparse"):
+            raise ValueError("storage must be 'auto', 'dense' or 'sparse', got %r" % (self.storage,))
         eng = self.engine
         t0 = time.perf_counter()
         idx_d = eng.upload(np.ascontiguousarray(_as_index_array(idx)))
         a = eng.coo_to_csr(idx_d[:, 0], idx_d[:, 1], eng.upload(_as_value_array(val)), shape)
-        self._i2i_dev = eng.cooc_build(a, implicit=self.implicit)
+        self._i2i_dev = self._i2i_csr = None
+        if self.storage != "sparse":
+            try:
+                self._i2i_dev = eng.cooc_build(a, implicit=self.implicit)
+            except MemoryError:
+                if self.storage == "dense":
+                    raise
+        if self._i2i_dev is None:
+            self._i2i_csr = eng.cooc_build_csr(a, implicit=self.implicit)
+        self.i2i_storage = "dense" if self._i2i_dev is not None else "sparse"
         self._i2i_items = int(shape[1])
         eng.sync()
         t1 = time.perf_counter()
@@ -1266,12 +1285,25 @@ class _CooccurrenceDeviceMixin(_DeviceModelMixin):
             out[a:b] = dense[a:b] if is_dense else sparse[a:b]
         return out
 
+    def _scoring_csr(self):
+        """the fp64 CSR the sparse form scores with (P S_csr), or None for the dense form"""
+        return self._i2i_csr
+
+    def _scoring_test_csr(self, test_data, shape):
+        return self._test_csr_device(test_data, shape)
+
     def i2i_lists(self, test_data, shape):
-        """``(nnz_u, dense-rule lists, sparse-rule lists)`` of the test users, as numpy arrays (pb200_i2i_topk)."""
+        """``(nnz_u, dense-rule lists, sparse-rule lists)`` of the test users, as numpy arrays (pb200_i2i_topk or, for
+        the sparse form, pb200_i2i_topk_csr)."""
         eng = self.engine
-        p_dev, seen_dev = self._test_csr_device(test_data, shape)
-        nnz, dense, sparse = eng.i2i_topk(self._i2i_dev, self._i2i_items, p_dev, self.topk,
-                                          seen=seen_dev if self.filter_seen else None, implicit=self.implicit)
+        p_dev, seen_dev = self._scoring_test_csr(test_data, shape)
+        seen = seen_dev if self.filter_seen else None
+        s_csr = self._scoring_csr()
+        if s_csr is None:
+            nnz, dense, sparse = eng.i2i_topk(self._i2i_dev, self._i2i_items, p_dev, self.topk, seen=seen,
+                                              implicit=self.implicit)
+        else:
+            nnz, dense, sparse = eng.i2i_topk_csr(s_csr, p_dev, self.topk, seen=seen, implicit=self.implicit)
         return nnz.cpu().numpy(), dense.cpu().numpy(), sparse.cpu().numpy()
 
 
@@ -1302,6 +1334,90 @@ def dropin_i2i():
             return _CooccurrenceDeviceMixin.build(self)
 
     return PolaraB200Cooccurrence
+
+
+class _SimilarityDeviceMixin(_CooccurrenceDeviceMixin):
+    """Device implementation of SimilarityAggregation (hybrid/models.py:25-44): the item relations of the data model
+    with a zero diagonal and no stored zeros, scored as ``sparse_dot(P, S)`` -- ``P S^T`` (lib/sparse.py:48), so the
+    device holds S^T as an fp64 CSR -- under the chunk rules of the item-to-item model.  With ``dense_output`` the
+    reference multiplies through ``csc_matvec`` (lib/sparse.py:40-43), which reads the stored arrays of S as CSC: that
+    is ``P S`` for relations held as CSR and ``P S^T`` for any other format, and the device follows it.  ``implicit``
+    scores with ones for every nonzero test feedback (hybrid/models.py:41-42)."""
+
+    def build(self):
+        rel = self.data.item_relations.copy()        # the copy keeps the data model's matrix intact (:33)
+        rel.setdiag(0)
+        rel.eliminate_zeros()
+        self.item_similarity_matrix = rel
+        self._i2i_dev = None
+        self._i2i_items = int(rel.shape[1])
+        self._sim_forms = {}
+        self._sim_operand_is_s = getattr(rel, "format", None) == "csr"
+        self.i2i_storage = "sparse"
+
+    def _scoring_csr(self):
+        """S^T, or S for ``dense_output`` on CSR relations, as a device fp64 CSR (uploaded once per form)."""
+        import scipy.sparse as sps
+        use_s = bool(self.dense_output) and self._sim_operand_is_s
+        hit = self._sim_forms.get(use_s)
+        if hit is None:
+            rel = self.item_similarity_matrix
+            mat = sps.csr_matrix(rel if use_s else rel.T, dtype=np.float64)
+            mat.sum_duplicates()
+            mat.sort_indices()
+            eng = self.engine
+            hit = DeviceCSR(eng.upload(mat.indptr.astype(np.int64)), eng.upload(mat.indices.astype(np.int32)),
+                            eng.upload(mat.data.astype(np.float64)), mat.shape)
+            self._sim_forms[use_s] = hit
+        return hit
+
+    def _scoring_test_csr(self, test_data, shape):
+        if not self.implicit:
+            return self._test_csr_device(test_data, shape)
+        user, item, fdbk = test_data
+        # ones for the nonzero feedback; zero feedback is still dropped (get_test_matrix, models.py:197-201)
+        ones = (np.asarray(fdbk) != 0).astype(np.float64)
+        return self._test_csr_device((user, item, ones), shape)
+
+    def i2i_lists(self, test_data, shape):
+        eng = self.engine
+        p_dev, seen_dev = self._scoring_test_csr(test_data, shape)
+        seen = seen_dev if self.filter_seen else None
+        # with ``implicit`` the values are already 1 (or a count of duplicate triplets, whose sign is 1)
+        nnz, dense, sparse = eng.i2i_topk_csr(self._scoring_csr(), p_dev, self.topk, seen=seen, implicit=self.implicit)
+        return nnz.cpu().numpy(), dense.cpu().numpy(), sparse.cpu().numpy()
+
+
+class B200SimilarityAggregation(_SimilarityDeviceMixin, host.RecommenderModel):
+    """Stand-alone SimilarityAggregation (hybrid/models.py:25-44) on a data model that carries ``item_relations``
+    (``host.ArrayData(..., item_relations=...)``)."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.method = "SIM"
+        self.implicit = False
+        self.dense_output = False
+        self.item_similarity_matrix = False
+
+    def build(self):
+        return _SimilarityDeviceMixin.build(self)
+
+
+def dropin_similarity():
+    """``PolaraB200SimilarityAggregation``: the device scorer on the REAL ``polara`` SimilarityAggregation (data models
+    with item relations, e.g. SimilarityDataModel); the chunk rules read ``polara.recommender.defaults.memory_hard_limit``
+    as the reference does."""
+    from polara.recommender import defaults
+    from polara.recommender.hybrid.models import SimilarityAggregation
+
+    class PolaraB200SimilarityAggregation(_SimilarityDeviceMixin, SimilarityAggregation):
+        def _memory_hard_limit(self):
+            return defaults.memory_hard_limit
+
+        def build(self):
+            return _SimilarityDeviceMixin.build(self)
+
+    return PolaraB200SimilarityAggregation
 
 
 def dropin():
