@@ -28,6 +28,7 @@
 //                          in 64 fp32 registers per thread, releases each ring stage as soon as its MMAs retired, then
 //                          turns the signs into per-user candidate masks, stages them and rescores.
 #include <cuda_bf16.h>
+#include <cfloat>
 #include <cstdlib>
 #include <cub/device/device_radix_sort.cuh>
 
@@ -192,8 +193,11 @@ __device__ __forceinline__ uint32_t pack_threshold(float t) {
     if (!(t > -3.0e38f)) t = -3.0e38f;
     // explicit slack for the fp32 accumulation inside the tensor core (<= 67 additions, each 2^-24 relative to a partial sum
     // of size <= |t| + ||e|| ||v||): the |t| share is taken off the threshold here (2^-16 |t| >= 67 * 2^-24 |t|), the other share
-    // is in the margin factor (pack_users_kernel)
-    t -= fabsf(t) * 1.52587890625e-5f;
+    // is in the margin factor (pack_users_kernel).  FLT_MIN more puts the threshold strictly below a score of 0: where the
+    // margin product is 0 (an item of norm 0, or ||e|| ||v|| 2^-7 under the accumulator's range) the accumulator would
+    // otherwise sum to +0, and an item whose exact score ties a k-th score of 0 (and wins on its id) would not fire.  For
+    // |t| >= 2^-86 the FLT_MIN is absorbed.
+    t -= fabsf(t) * 1.52587890625e-5f + FLT_MIN;
     uint32_t hi = bf16_floor_bits(t);
     float hif = __uint_as_float(hi << 16);
     float rem = t - hif;                          // >= 0, exact
@@ -556,7 +560,9 @@ probe_kernel(const float* __restrict__ E, int64_t lde, const float* __restrict__
                 const int pos = lane + 32 * j;
                 const uint32_t w = __shfl_sync(0xffffffffu, seen_w[a], j);
                 const bool ok = act[a] && pos < n_probe && !(w & (0x80000000u >> lane));
-                ord[a][j] = ok ? ord_of(sm.sc[act[a] ? ul + 8 * a : 0][pos]) : 0u;
+                // + 0.f turns -0 into +0: the two zeros tie and the id decides, as in cand_before (ord_of alone puts -0
+                // below +0); the sign of a zero score is restored after the selection
+                ord[a][j] = ok ? ord_of(sm.sc[act[a] ? ul + 8 * a : 0][pos] + 0.f) : 0u;
                 lmax[a] = max(lmax[a], ord[a][j]);
             }
         }
@@ -592,11 +598,14 @@ probe_kernel(const float* __restrict__ E, int64_t lde, const float* __restrict__
         for (int a = 0; a < PNU; ++a) fast[a] = act[a] && small_k && count[a] <= 32;
         __syncwarp();
         unsigned long long mine[PNU];
+        uint32_t mpos[PNU];                                                    // probe position of this lane's key
 #pragma unroll
         for (int a = 0; a < PNU; ++a) {
             mine[a] = 0ull;
+            mpos[a] = 0u;
             if (fast[a] && lane < count[a]) {
                 const unsigned long long c = sm.cand[warp][a][lane];
+                mpos[a] = (uint32_t)c;
                 const uint32_t id = (uint32_t)__ldg(perm + (uint32_t)c);
                 mine[a] = (c & 0xFFFFFFFF00000000ull) | (unsigned long long)(0xFFFFFFFFu - id);
             }
@@ -613,6 +622,7 @@ probe_kernel(const float* __restrict__ E, int64_t lde, const float* __restrict__
             for (int t = 0; t < count[a]; ++t) rank += sm.cand[warp][a][t] > mine[a] ? 1 : 0;
             if (lane < count[a] && rank < k) {
                 pb200_cand c; c.score = ord_to_float((uint32_t)(mine[a] >> 32)); c.id = (int)(0xFFFFFFFFu - (uint32_t)mine[a]);
+                if (c.score == 0.f) c.score = sm.sc[ul + 8 * a][mpos[a]];  // the key ranked -0 as +0: the canonical sign
                 out[rank] = c;
                 if (rank == k - 1) sm.t0s[ul + 8 * a] = c.score;
             }
@@ -632,6 +642,18 @@ probe_kernel(const float* __restrict__ E, int64_t lde, const float* __restrict__
                 key[j] = ord[a][j] ? (((unsigned long long)ord[a][j] << 32) | (unsigned long long)(0xFFFFFFFFu - id)) : 0ull;
             }
             probe_select_rounds<PL>(key, lane, k, out_list + u[a] * k, &sm.t0s[ul + 8 * a]);
+        }
+        // the reference selection's keys ranked a -0 score as +0 and carry no position: a zero score is recomputed, so that
+        // its sign is the canonical one (the fast path restored it from the score tile above)
+        __syncwarp();
+#pragma unroll
+        for (int a = 0; a < PNU; ++a) {
+            if (!act[a] || fast[a]) continue;
+            pb200_cand* out = out_list + u[a] * k;
+            for (int j = lane; j < k; j += 32) {
+                const pb200_cand c = out[j];
+                if (c.id >= 0 && c.score == 0.f) out[j].score = exact_score(E + u[a] * lde, V + (int64_t)c.id * ldv, r);
+            }
         }
     }
     __syncthreads();

@@ -16,9 +16,13 @@ class ItemShard:
 
     def __init__(self, rank, world, n_items):
         self.rank, self.world, self.n_items = int(rank), int(world), int(n_items)
-        per = (self.n_items + self.world - 1) // self.world
-        self.item_lo = min(self.n_items, self.rank * per)
-        self.item_hi = min(self.n_items, (self.rank + 1) * per)
+        # balanced ranges (sizes differ by at most one): with n_items >= world no rank is left without items, which the
+        # scoring kernels refuse (a ceil-sized split gives n = 13, world = 8 the empty range [13, 13) on rank 7)
+        if self.n_items < self.world:
+            raise ValueError("ItemShard: %d items cannot be split over %d ranks (every rank needs at least one item)"
+                             % (self.n_items, self.world))
+        self.item_lo = self.rank * self.n_items // self.world
+        self.item_hi = (self.rank + 1) * self.n_items // self.world
 
     def user_chunk(self, n_users):
         """users are split into `world` equal chunks (the last ones may be short/padded)."""

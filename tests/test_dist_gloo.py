@@ -25,6 +25,15 @@ def test_item_shard_bounds_cover_everything():
         assert covered == n_users
 
 
+def test_item_shard_never_empty_and_refuses_more_ranks_than_items():
+    for world, n in ((8, 13), (8, 8), (3, 4), (7, 100), (1, 2)):
+        shards = [ItemShard(r, world, n) for r in range(world)]
+        assert all(s.item_hi > s.item_lo for s in shards)
+        assert max(s.item_hi - s.item_lo for s in shards) - min(s.item_hi - s.item_lo for s in shards) <= 1
+    with pytest.raises(ValueError):
+        ItemShard(0, 8, 7)
+
+
 def _free_port():
     with socket.socket() as s:
         s.bind(("127.0.0.1", 0))
