@@ -97,6 +97,97 @@ class ArrayData:
                    n_feedback=int(g["train_shape"][2]) if tensor else None)
 
 
+_ItemColdIndex = namedtuple("ItemIndex", "training cold_start")
+
+
+class ColdStartData:
+    """Stand-alone item cold-start data model: what ``ItemColdStartData`` (coldstart/data.py:10-224) hands to the SVD
+    family's cold-start models once its split is made.  Splitting, reindexing and the one-hot encoding of DataFrame
+    features are out of scope; the caller passes arrays in the model's index:
+
+    * ``train_idx`` [nnz x 2] (user, item), ``train_val``, ``train_shape``: the training triplets of the warm items;
+    * ``cold_item``, ``cold_user``, ``cold_fdbk``: the holdout, every interaction of the cold items, by cold id;
+    * ``item_features`` F [n_items x n_features] and ``cold_item_features`` F_cold [n_cold x n_features] (row = cold
+      id): one-hot features of the training and the cold items in one column space;
+    * ``n_users``: the training users (the columns of the cold items' lists);
+    * ``representative_users``: optional user ids (data.py:37-46).
+
+    The rules of the reference's post-processing (data.py:128-217) are applied here:
+
+    * the cold items are those with holdout rows;
+    * a cold item none of whose features a training item has is dropped, with its holdout rows (data.py:162-185);
+    * with ``representative_users``, when some cold item has no holdout row of a representative user, that item is
+      dropped and the holdout keeps the representative users' rows only; when every cold item has one, the holdout
+      stays whole (data.py:143-160, 187-210: the filter is only set up for items that lack one);
+    * features no training item has are dropped from F_cold (``stack_features`` with the training labels drops
+      unknown labels, similarity.py:259-267);
+    * the holdout is sorted by cold id (data.py:212-217); ``index.itemid.cold_start`` holds the kept cold ids in
+      ascending order, and ``cold_item_features`` their rows in that order.
+
+    Scoring still ranks every training user for a cold item; the representative users only filter the holdout."""
+
+    on_change_event = "on_change"
+    on_update_event = "on_update"
+
+    def __init__(self, train_idx, train_val, train_shape, cold_item, cold_user, cold_fdbk, item_features,
+                 cold_item_features, n_users=None, representative_users=None, fields=("userid", "itemid", "rating")):
+        import pandas as pd
+        import scipy.sparse as sps
+        self.fields = Fields(*fields)
+        self._train = (np.asarray(train_idx), np.asarray(train_val), tuple(int(s) for s in train_shape))
+        n_users = self._train[2][0] if n_users is None else int(n_users)
+        f = sps.csr_matrix(item_features, dtype=np.float64)
+        fc = sps.csr_matrix(cold_item_features, dtype=np.float64)
+        if f.shape[0] != self._train[2][1] or fc.shape[1] != f.shape[1]:
+            raise ValueError("item features must be [n_items x n_features] (%d items) and cold item features share their "
+                             "columns; got %s and %s" % (self._train[2][1], f.shape, fc.shape))
+        seen_cols = np.zeros(f.shape[1], dtype=bool)
+        seen_cols[f.indices[f.data != 0]] = True
+        fc = fc.multiply(seen_cols[None, :].astype(np.float64)).tocsr()      # unknown features dropped
+        fc.eliminate_zeros()
+        cold_item, cold_user = np.asarray(cold_item, dtype=np.int64), np.asarray(cold_user, dtype=np.int64)
+        cold_fdbk = np.asarray(cold_fdbk)
+        present = np.bincount(cold_item, minlength=fc.shape[0]) > 0          # the cold index comes from the holdout
+        keep_item = present & (np.diff(fc.indptr) > 0)                       # shares a feature with a training item
+        keep_row = keep_item[cold_item]
+        if representative_users is not None:
+            representative_users = np.unique(np.asarray(representative_users, dtype=np.int64))
+            is_repr_row = np.isin(cold_user, representative_users)
+            has_repr = np.zeros(fc.shape[0], dtype=bool)
+            has_repr[cold_item[is_repr_row]] = True
+            if not has_repr[present].all():          # data.py:158-159, 198-201: only then is the holdout filtered
+                keep_item &= has_repr
+                keep_row &= is_repr_row & keep_item[cold_item]
+        order = np.argsort(cold_item[keep_row], kind="stable")
+        cold_col = "%s_cold" % self.fields.itemid
+        self.test = _Test(None, pd.DataFrame({self.fields.userid: cold_user[keep_row][order],
+                                              cold_col: cold_item[keep_row][order],
+                                              self.fields.feedback: cold_fdbk[keep_row][order]}))
+        cold_ids = np.flatnonzero(keep_item)
+        self.item_features = f
+        self.cold_item_features = fc[cold_ids]
+        self.representative_users = representative_users
+        self.index = _Index(np.arange(n_users), _ItemColdIndex(np.arange(self._train[2][1]), cold_ids), None)
+        self.warm_start = False
+        self.holdout_size = -1
+        self.test_sample = None
+        self.train_csr = None
+        self.test_csr = None
+        self._subscribers = []
+
+    def subscribe(self, event, callback):
+        self._subscribers.append((event, callback))
+
+    def to_coo(self, tensor_mode=False, feedback_threshold=None):
+        idx, val, shp = self._train
+        if tensor_mode:
+            raise ValueError("ColdStartData holds 2-way training indices")
+        if feedback_threshold is not None:
+            keep = val >= feedback_threshold          # data.py:783-788 (filter_values=True)
+            idx, val = idx[keep], val[keep]
+        return idx.astype(np.intp, copy=False), np.ascontiguousarray(val), shp
+
+
 # ------------------------------------------------------------------ metrics -------
 Hits = namedtuple("Hits", "true_positive false_positive true_negative false_negative")
 Relevance = namedtuple("Relevance", "precision recall fallout specifity miss_rate")
@@ -407,16 +498,30 @@ class RecommenderModel:
         switch_positive = switch_positive or self.switch_positive
         f = self.data.fields
         holdout = self.data.test.holdout
-        h_user = np.asarray(holdout[f.userid].values, dtype=np.int64)
-        h_item = np.asarray(holdout[self._prediction_target].values, dtype=np.int64)     # assemble_scoring_matrices
+        # assemble_scoring_matrices (models.py:445-446): lists are matched by the holdout's key and target columns --
+        # (user, item) pairs, or (cold item, user) pairs in item cold start
+        h_user = np.asarray(holdout[self._prediction_key].values, dtype=np.int64)
+        h_item = np.asarray(holdout[self._prediction_target].values, dtype=np.int64)
         h_fdbk = None if (f.feedback is None or ignore_feedback) else np.asarray(holdout[f.feedback].values)
         if f.feedback is None:
             switch_positive = None
         fd_for_pos = None if f.feedback is None else np.asarray(holdout[f.feedback].values)
         res = evaluate_lists(recommendations, h_user, h_item,
                              fd_for_pos if h_fdbk is None and switch_positive is not None else h_fdbk,
-                             self.data.index.itemid.shape[0], metric_type=metric_type,
+                             self._target_entity_count(), metric_type=metric_type,
                              switch_positive=switch_positive, not_rated_penalty=not_rated_penalty,
                              ndcg_alternative=DEFAULTS["ndcg_alternative"],
                              simple_rates=simple_rates or getattr(self.data, "holdout_size", None) == 1)
         return res
+
+    def _target_entity_count(self):
+        """the coverage denominator (models.py:465-471): the size of the index of the entity the lists hold -- items, or
+        the training users in item cold start.  A target that is not a field (the holdout positions of sampled
+        evaluation) counts the items."""
+        fields = self.data.fields
+        target = self._prediction_target if self._prediction_target in fields else fields.itemid
+        entity_index = getattr(self.data.index, fields._fields[fields.index(target)])
+        try:
+            return entity_index.shape[0]
+        except AttributeError:
+            return entity_index.training.shape[0]

@@ -11,6 +11,9 @@ Two families of classes share the device logic (mixins below):
   mirror base in :mod:`polara_b200.host` (works without the reference installed);
 * :func:`dropin` -- the same mixins grafted onto the *real* ``polara`` classes when that
   package is importable, so that ``polara.evaluation`` pipelines keep working unchanged.
+
+The HybridSVD, item-to-item, SimilarityAggregation and item cold-start models follow the same pattern
+(``dropin_hybrid``, ``dropin_i2i``, ``dropin_similarity``, ``dropin_coldstart``).
 """
 from __future__ import annotations
 
@@ -23,8 +26,9 @@ from . import host
 from .engine import DeviceCSR, get_engine, round_up
 
 __all__ = ["B200SVDModel", "B200ScaledSVD", "B200HybridSVD", "B200ScaledHybridSVD", "B200CoffeeModel",
-           "B200CooccurrenceModel", "B200SimilarityAggregation", "dropin", "dropin_hybrid", "dropin_i2i",
-           "dropin_similarity", "default_ell"]
+           "B200CooccurrenceModel", "B200SimilarityAggregation", "B200SVDModelItemColdStart",
+           "B200ScaledSVDItemColdStart", "B200HybridSVDItemColdStart", "B200ScaledHybridSVDItemColdStart", "dropin",
+           "dropin_coldstart", "dropin_hybrid", "dropin_i2i", "dropin_similarity", "default_ell"]
 
 
 def default_ell(rank, oversample=None):
@@ -669,19 +673,37 @@ class _SVDDeviceMixin(_DeviceModelMixin):
         u = self.factors.get(f.userid, None)
         if u is None:
             raise ValueError("cold start needs the user factors: build(return_factors=True)")
-        s = np.asarray(self.factors["singular_values"])
         r = u.shape[1]
         w = np.asarray(feature_embeddings)[:, :r] @ np.asarray(transform_helper)[:r, :r]      # fold the r x r map into W
         fc = sps_.csr_matrix(cold_item_features)
         fc.sort_indices()
         ld = round_up(r, 32)
         w_pad = np.zeros((w.shape[0], ld), dtype=np.float32); w_pad[:, :r] = w
-        us = np.zeros((u.shape[0], ld), dtype=np.float32); us[:, :r] = u * s[None, :r]
-        f_dev = eng.upload_csr(fc.indptr.astype(np.int64), fc.indices.astype(np.int32), fc.data.astype(np.float32), fc.shape)
-        e = eng.spmm(f_dev, eng.upload(w_pad), ell=ld)                      # cold item factors [n_cold x r]
         if self.topk > u.shape[0]:
             raise ValueError("topk exceeds the number of users")
-        return eng.score_topk(e, eng.upload(us), r, self.topk, seen=None).cpu().numpy()
+        us_dev = self._device_scaled_users()
+        f_dev = eng.upload_csr(fc.indptr.astype(np.int64), fc.indices.astype(np.int32), fc.data.astype(np.float32), fc.shape)
+        with eng.score_kernel_scope(self.score_kernel):
+            e = eng.spmm(f_dev, eng.upload(w_pad), ell=ld)                  # cold item factors [n_cold x r]
+            return eng.score_topk(e, us_dev, r, self.topk, seen=None).cpu().numpy()
+
+    def _device_scaled_users(self):
+        """``U diag(sigma)`` on the device, zero padded to a multiple of 32 columns, at the width of the arrays it was
+        formed from; cached like ``_device_factor``.  Rank truncation (models.py:819-832) replaces U and sigma by their
+        leading columns, views of the same arrays, so the cached operand serves every lower rank without an upload: its
+        leading r columns are the truncated product's bits, and the scoring kernel reads r columns only."""
+        f = self.data.fields
+        u = np.asarray(self.factors[f.userid])
+        s = np.asarray(self.factors["singular_values"])
+        hit = self.__dict__.get("_dev_scaled_users")
+        if hit is not None and _leading_columns_of(u, hit[0]) and _leading_columns_of(s, hit[1]):
+            return hit[2]
+        r = u.shape[1]
+        us = np.zeros((u.shape[0], round_up(r, 32)), dtype=np.float32)
+        us[:, :r] = u * s[None, :r]
+        dev = self.engine.upload(us)
+        self._dev_scaled_users = (u, s, dev)
+        return dev
 
     def slice_recommendations(self, test_data, shape, start, stop, test_users=None):
         """Dense score rows for a (small) user slice -- kept for the single-user helpers
@@ -696,6 +718,19 @@ class _SVDDeviceMixin(_DeviceModelMixin):
         e = eng.spmm(p_dev, v_dev, ell=r_live)
         s = eng.score_dense(e, v_dev, r_live)
         return s.cpu().numpy().astype(np.float64), sl
+
+
+def _leading_columns_of(view, full):
+    """True when ``view`` is ``full`` or ``full[..., :r]`` (what rank truncation makes of a factor, models.py:819-832):
+    same memory start, same strides and leading dimensions, no wider."""
+    if view is full:
+        return True
+    # numpy points a view at the array that owns the memory, or at ``full`` when ``full`` wraps a foreign buffer
+    # (``Tensor.numpy()``)
+    same_owner = view.base is full or (full.base is not None and view.base is full.base)
+    return (same_owner and view.shape[:-1] == full.shape[:-1] and view.shape[-1] <= full.shape[-1]
+            and view.strides == full.strides
+            and view.__array_interface__["data"][0] == full.__array_interface__["data"][0])
 
 
 def sampled_exclusion_lists(test_data, shape, holdout_items, holdout_users=None):
@@ -1003,6 +1038,144 @@ class B200HybridSVD(_HybridSVDDeviceMixin, _SVDState, host.RecommenderModel):
 
 class B200ScaledHybridSVD(_ScaledMatrixMixin, B200HybridSVD):
     """ScaledHybridSVD (hybrid/models.py:397): HybridSVD on the scaled training matrix."""
+
+
+# ------------------------------------------------------------------ item cold start ----------
+class _ItemColdStartMixin:
+    """Item cold start on the SVD family: a restatement of polara/recommender/coldstart/models.py, whose module cannot be
+    imported without ``lightfm`` (its line 8 imports LightFMWrapper).  It composes, in this order:
+
+    * ItemColdStartEvaluationMixin (:13-18): nothing is seen, and the lists are matched as (cold item, user) pairs:
+      ``_prediction_key = '<itemid>_cold'``, ``_prediction_target = userid``;
+    * ItemColdStartRecommenderMixin (:21-52): one row per cold item of ``index.itemid.cold_start``, the top-k users;
+    * ItemColdStartSVDModelMixin (:149-222): the build with the user factors, then the feature mapping
+      ``W = F^T V`` (``<itemid>_features`` in ``factors``, so rank truncation cuts it with the rest) and its transform
+      ``pinv(W^T W)``, both once per build on the host in float64.  Scores are ``(F_cold W) pinv(W^T W) (U diag s)^T``.
+
+    The device work is the parent's build and ``coldstart_recommendations`` (pb200_spmm_csr for the cold items' factors,
+    pb200_score_topk over the users).  ``_mapping_source`` names the factor W is built from: the item factors V
+    (SVDModelItemColdStart, :233-236) or HybridSVD's right item projector (HybridSVDItemColdStart, :247-251).
+
+    Features: a DataFrame of per-item label lists (the reference's form, one-hot encoded by polara's ``stack_features``),
+    or, with :class:`polara_b200.host.ColdStartData`, the data model's F and F_cold."""
+
+    _mapping_source = "{}"
+
+    def __init__(self, *args, item_features=None, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.filter_seen = False                      # there are no seen entities in cold start
+        self._prediction_key = "{}_cold".format(self.data.fields.itemid)
+        self._prediction_target = self.data.fields.userid
+        if item_features is None:                     # features are provided via the data model
+            item_features = self.data.item_features
+        assert item_features is not None
+        self.item_features = item_features
+        self.item_features_labels = None
+        self._item_features_transform_helper = None
+        self.data.subscribe(self.data.on_change_event, self._clean_metadata)
+
+    def _clean_metadata(self):
+        self.item_features_labels = None
+
+    @property
+    def item_features_embeddings(self):
+        return self.factors.get("{}_features".format(self.data.fields.itemid), None)
+
+    def _round_item_features_transform(self):
+        try:
+            rank = self.item_features_embeddings.shape[1]
+        except AttributeError:                        # embeddings are None (not built, or cleared by a higher rank)
+            self._item_features_transform_helper = None
+        else:
+            if self._item_features_transform_helper.shape[0] > rank:
+                self.update_item_features_transform()
+            else:
+                raise ValueError("Unable to round: the rank of factors is not lower than the rank of transform!")
+
+    def _check_reduced_rank(self, rank):
+        super()._check_reduced_rank(rank)
+        self._round_item_features_transform()
+
+    def _features_given_as_matrix(self):
+        import scipy.sparse as sps_
+        return sps_.issparse(self.item_features)
+
+    def encode_item_features(self):
+        """the training items' one-hot F (:185-190)."""
+        if self._features_given_as_matrix():
+            return self.item_features
+        from polara.lib.similarity import stack_features
+        training_items = self.data.index.itemid.training.old.values
+        item_features = self.item_features.reindex(training_items, fill_value=[])
+        item_one_hot, self.item_features_labels = stack_features(item_features, stacked_index=False, normalize=False)
+        return item_one_hot
+
+    def encode_cold_item_features(self):
+        """F_cold in the order of ``index.itemid.cold_start``, features unseen in training dropped (:26-29, 210-214)."""
+        if self._features_given_as_matrix():
+            return self.data.cold_item_features
+        from polara.lib.similarity import stack_features
+        cold_item_meta = self.item_features.reindex(self.data.index.itemid.cold_start.old.values, fill_value=[])
+        cold_item_features, _ = stack_features(cold_item_meta, labels=self.item_features_labels, normalize=False)
+        return cold_item_features
+
+    def compute_item_features_mapping(self, item_features):
+        return item_features.T.dot(self.factors[self._mapping_source.format(self.data.fields.itemid)])
+
+    def update_item_features_transform(self):
+        mapping = self.item_features_embeddings
+        self._item_features_transform_helper = np.linalg.pinv(mapping.T @ mapping)
+
+    def prepare_item_features_transformation(self):
+        item_one_hot = self.encode_item_features()
+        self.factors["{}_features".format(self.data.fields.itemid)] = self.compute_item_features_mapping(item_one_hot)
+        self.update_item_features_transform()
+
+    def build(self, *args, **kwargs):
+        super().build(*args, return_factors=True, **kwargs)
+        self.prepare_item_features_transformation()
+
+    def get_recommendations(self):
+        if self.verify_integrity and hasattr(self, "verify_data_integrity"):
+            self.verify_data_integrity()
+        return self.coldstart_recommendations(self.encode_cold_item_features(), self.item_features_embeddings,
+                                              self._item_features_transform_helper)
+
+
+class _HybridColdStartSource:
+    _mapping_source = "{}_projector_right"
+
+
+class B200SVDModelItemColdStart(_ItemColdStartMixin, B200SVDModel):
+    """SVDModelItemColdStart (coldstart/models.py:225-236) on :class:`polara_b200.host.ColdStartData`."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.method = "PureSVD(cs)"
+
+    def build(self, *args, **kwargs):
+        return _ItemColdStartMixin.build(self, *args, **kwargs)
+
+
+class B200ScaledSVDItemColdStart(_ScaledMatrixMixin, B200SVDModelItemColdStart):
+    """ScaledSVDItemColdStart (coldstart/models.py:254)."""
+
+
+class B200HybridSVDItemColdStart(_HybridColdStartSource, _ItemColdStartMixin, B200HybridSVD):
+    """HybridSVDItemColdStart (coldstart/models.py:239-251): W is built from the right item projector, so a model
+    without an item Cholesky factor (no projectors) has nothing to map the features with and raises KeyError, as the
+    reference does."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.method = "HybridSVD(cs)"
+
+    def build(self, *args, **kwargs):
+        return _ItemColdStartMixin.build(self, *args, **kwargs)
+
+
+class B200ScaledHybridSVDItemColdStart(_ScaledMatrixMixin, B200HybridSVDItemColdStart):
+    """ScaledHybridSVDItemColdStart (coldstart/models.py:257)."""
 
 
 # ------------------------------------------------------------------ CoFFee ----------
@@ -1456,6 +1629,42 @@ def dropin_hybrid():
             return _HybridSVDDeviceMixin.build(self, return_factors=return_factors)
 
     return PolaraB200HybridSVD, PolaraB200ScaledHybridSVD
+
+
+def dropin_coldstart():
+    """``(PolaraB200SVDModelItemColdStart, PolaraB200ScaledSVDItemColdStart, PolaraB200HybridSVDItemColdStart,
+    PolaraB200ScaledHybridSVDItemColdStart)``: the item cold-start models on the REAL ``polara`` SVDModel, ScaledSVD,
+    HybridSVD and ScaledHybridSVD, for polara's ``ItemColdStartData`` (with item relations for the HybridSVD pair, e.g.
+    ``ItemColdStartSimilarityData``).  ``polara.recommender.coldstart.models`` is not imported, so ``lightfm`` need not be
+    installed; the features are one-hot encoded by polara's own ``stack_features``."""
+    from polara.recommender.hybrid.models import HybridSVD
+    from polara.recommender.models import ScaledMatrixMixin, SVDModel
+
+    class PolaraB200SVDModelItemColdStart(_ItemColdStartMixin, _SVDDeviceMixin, SVDModel):
+        def __init__(self, *args, **kwargs):
+            super().__init__(*args, **kwargs)
+            self.method = "PureSVD(cs)"
+
+        def build(self, *args, **kwargs):
+            return _ItemColdStartMixin.build(self, *args, **kwargs)
+
+    class PolaraB200ScaledSVDItemColdStart(ScaledMatrixMixin, PolaraB200SVDModelItemColdStart):
+        pass
+
+    class PolaraB200HybridSVDItemColdStart(_HybridColdStartSource, _ItemColdStartMixin, _HybridSVDDeviceMixin,
+                                           HybridSVD):
+        def __init__(self, *args, **kwargs):
+            super().__init__(*args, **kwargs)
+            self.method = "HybridSVD(cs)"
+
+        def build(self, *args, **kwargs):
+            return _ItemColdStartMixin.build(self, *args, **kwargs)
+
+    class PolaraB200ScaledHybridSVDItemColdStart(ScaledMatrixMixin, PolaraB200HybridSVDItemColdStart):
+        pass
+
+    return (PolaraB200SVDModelItemColdStart, PolaraB200ScaledSVDItemColdStart, PolaraB200HybridSVDItemColdStart,
+            PolaraB200ScaledHybridSVDItemColdStart)
 
 
 def dropin_sampled():

@@ -5,7 +5,8 @@
 The reference recomputes the recommendations at every rank; here they come from one call made before the loop --
 ``rank_sweep`` for the standard protocol, ``sampled_rank_sweep`` for sampled evaluation -- which shares the test-data
 ingest, the SpMM at the largest rank and, on the sampled protocol, the draw of the unseen items between all ranks.  The
-evaluator then sees the model at each rank with ``_recommendations`` set to that rank's lists.
+evaluator then sees the model at each rank with ``_recommendations`` set to that rank's lists.  Item cold-start models
+(users as the target) have a feature transform per rank and take the reference's per-rank loop instead.
 """
 from __future__ import annotations
 
@@ -45,13 +46,36 @@ def evaluate_models(models, target_metric="precision", metric_type="all", **kwar
 
 
 def rank_sweep_lists(model, ranks):
-    """``{rank: lists}`` of ``model.recommendations`` at every rank, from one sweep: the sampled protocol when the model
-    predicts holdout positions (``_prediction_target`` other than the item field; inputs read from the data model as
-    the sampled drop-in's ``get_recommendations`` reads them), the standard one otherwise."""
-    if model._prediction_target == model.data.fields.itemid:
+    """``{rank: lists}`` of ``model.recommendations`` at every rank.  Items as the target: one standard sweep.  Users as
+    the target (item cold start): the reference's loop, ``model.rank = r`` then ``get_recommendations()`` with ranks
+    descending, because every rank has its own feature transform; the model's rank, factors and transform are restored
+    afterwards.  Anything else predicts holdout positions: one sampled sweep, its inputs read from the data model as the
+    sampled drop-in's ``get_recommendations`` reads them."""
+    fields = model.data.fields
+    if model._prediction_target == fields.itemid:
         return model.rank_sweep(ranks)
+    if model._prediction_target == fields.userid:
+        state = _rank_state(model)
+        try:
+            lists = {}
+            for rank in sorted(set(ranks), reverse=True):
+                model.rank = rank
+                lists[rank] = model.get_recommendations()
+            return lists
+        finally:
+            _restore_rank_state(model, state)
     holdout_items, unseen, kwargs = sampled_protocol_inputs(model)
     return model.sampled_rank_sweep(ranks, holdout_items, unseen, **kwargs)
+
+
+def _rank_state(model):
+    return model._rank, dict(model.factors), getattr(model, "_item_features_transform_helper", None)
+
+
+def _restore_rank_state(model, state):
+    model._rank, model.factors = state[0], dict(state[1])
+    if hasattr(model, "_item_features_transform_helper"):
+        model._item_features_transform_helper = state[2]
 
 
 def find_optimal_svd_rank(model, ranks, target_metric, return_scores=False, protect_factors=True, config=None,
@@ -70,7 +94,7 @@ def find_optimal_svd_rank(model, ranks, target_metric, return_scores=False, prot
         model.verbose = verbose
         model.build()
     if protect_factors:
-        svd_factors = dict(model.factors)
+        svd_state = _rank_state(model)       # the transform of a cold-start model goes with its factors
     res = {}
     try:
         lists = rank_sweep_lists(model, ranks)
@@ -81,8 +105,7 @@ def find_optimal_svd_rank(model, ranks, target_metric, return_scores=False, prot
             model._recommendations = None          # the next rank must not see this rank's lists
     finally:
         if protect_factors:
-            model._rank = svd_rank
-            model.factors = svd_factors
+            _restore_rank_state(model, svd_state)
         model.verbose = model_verbose
     scores = pd.Series(res)
     best_rank = scores.idxmax()
