@@ -175,6 +175,7 @@ def test_dense_list_equals_topk_dense_on_the_host_block(eng, filter_seen):
 
 
 def test_non_integer_lists_are_a_valid_topk_of_the_f64_scores(eng):
+    """fp32-representable non-integer data: the lists, counts and scores are those of the f64 oracle, bit for bit"""
     n_items, k = 900, 10
     a = training(800, n_items, 31, values="float")
     s_dev = eng.cooc_build(device_csr(eng, a))
@@ -182,17 +183,13 @@ def test_non_integer_lists_are_a_valid_topk_of_the_f64_scores(eng):
     shape = (400, n_items)
     users, items, fd = make_test_data(shape[0], n_items, 32, zero_fdbk=False)
     fd = (fd * 0.37).astype(np.float32).astype(np.float64)
-    _, dense, sparse = run_topk(eng, s_dev, n_items, users, items, fd, shape, k, True, False)
-    _, w_dense, w_sparse, full, seen = lists_from_oracle(s, users, items, fd, shape, k, True, False)
-    p = io.test_matrix(users, items, fd, shape)
-    tol = 2.0 ** -40 * np.abs(p).sum(axis=1).max() * np.abs(s).max()
-    for got, want in ((dense, w_dense), (sparse, w_sparse)):
-        assert ((got < 0) == (want < 0)).all()
-        rows = np.arange(shape[0])[:, None]
-        sg = np.where(got >= 0, full[rows, np.maximum(got, 0)], 0)
-        sw = np.where(want >= 0, full[rows, np.maximum(want, 0)], 0)
-        assert np.abs(sg - sw).max() <= tol            # position by position the same score up to near-ties
-    assert (dense == w_dense).mean() > 0.99
+    nnz, dense, sparse, scores = run_topk(eng, s_dev, n_items, users, items, fd, shape, k, True, False,
+                                          want_scores=True)
+    w_nnz, w_dense, w_sparse, full, _ = lists_from_oracle(s, users, items, fd, shape, k, True, False)
+    np.testing.assert_array_equal(nnz, w_nnz)
+    np.testing.assert_array_equal(dense, w_dense)
+    np.testing.assert_array_equal(sparse, w_sparse)
+    assert scores.tobytes() == np.take_along_axis(full, w_dense, axis=1).tobytes()
 
 
 def test_two_runs_give_identical_lists(eng):
@@ -253,13 +250,10 @@ def test_model_reproduces_the_reference_runs(eng, case):
     seen = sps.csr_matrix((np.ones(len(a["test_user"])), (a["test_user"], a["test_item"])), shape=a["test_shape"])
     flag = lambda x: np.array([np.isin(x[u], seen.indices[seen.indptr[u]:seen.indptr[u + 1]])   # noqa: E731
                                for u in range(x.shape[0])]) & (x >= 0)
-    if case == "float":
-        np.testing.assert_allclose(score(recs), score(ref), rtol=1e-12)
-        assert (recs == want).mean() > 0.99
-    else:
-        np.testing.assert_array_equal(score(recs), score(ref))
-        np.testing.assert_array_equal(recs, want)            # the oracle's tie rule fixes every id
-        np.testing.assert_array_equal(flag(recs), flag(want))
+    # exact on the float case too: its values are fp32-representable, so S and the scores have the reference's bits
+    np.testing.assert_array_equal(score(recs), score(ref))
+    np.testing.assert_array_equal(recs, want)                # the oracle's tie rule fixes every id
+    np.testing.assert_array_equal(flag(recs), flag(want))
 
 
 def test_topk_larger_than_the_catalogue_raises(eng):
