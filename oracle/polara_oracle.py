@@ -122,17 +122,25 @@ def hybrid_slice_scores(test_matrix, vl, vr):
 def rescale_matrix(matrix, scaling, axis):
     """preprocessing/matrices.py:71-93 with ``binary=True`` (the default used
     by ScaledMatrixMixin): scale rows (axis=1) or columns (axis=0) by
-    ``sqrt(nnz_count)**(scaling-1)``; zero-count lines keep an (irrelevant) factor."""
+    ``sqrt(count)**(scaling-1)``, ``count`` the line's stored entries
+    (``getnnz``: explicit zeros included); zero-count lines keep an
+    (irrelevant) factor.
+
+    There is no early return at ``scaling == 1``: the reference forms the
+    product with ``diags(...)`` then too, and a scipy sparse product stores
+    only nonzero results.  So the result never holds an explicit zero, and in
+    ``scaled_training_matrix`` the column counts, taken after the row pass,
+    exclude the zeros that the row counts include."""
     m = sps.csr_matrix(matrix, dtype=np.float64)
-    if scaling == 1:
-        return m
     counts = np.asarray(m.getnnz(axis=axis)).ravel()
     norm = np.sqrt(counts)
     factor = np.ones_like(norm)
     nz = norm != 0
     factor[nz] = np.power(norm[nz], scaling - 1)
     d = sps.diags(factor)
-    return (m @ d).tocsr() if axis == 0 else (d @ m).tocsr()
+    out = (m @ d).tocsr() if axis == 0 else (d @ m).tocsr()
+    out.eliminate_zeros()          # what the sparse product does; stated here rather than left to scipy
+    return out
 
 
 def scaled_training_matrix(matrix, row_scaling=1, col_scaling=0.4):

@@ -65,10 +65,13 @@ __global__ void indptr_from_sorted_kernel(const int32_t* __restrict__ sorted_key
     indptr[c] = lo;
 }
 
-__global__ void count_cols_kernel(const int32_t* __restrict__ indices, int64_t nnz, int32_t* __restrict__ counts) {
+// nonzero values per column: stored zeros (explicit zero feedback, duplicates that cancel) are not counted
+__global__ void count_cols_kernel(const int32_t* __restrict__ indices, const float* __restrict__ values, int64_t nnz,
+                                  int32_t* __restrict__ counts) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; i < nnz; i += stride) atomicAdd(counts + indices[i], 1);   // integer counts: order-independent
+    for (; i < nnz; i += stride)
+        if (values[i] != 0.0f) atomicAdd(counts + indices[i], 1);   // integer counts: order-independent
 }
 
 __global__ void rescale_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
@@ -84,7 +87,12 @@ __global__ void rescale_kernel(const int64_t* __restrict__ indptr, const int32_t
         if (do_rows && e > b) rf = pow(sqrt((double)(e - b)), row_pow);
         for (int64_t p = b + lane; p < e; p += 32) {
             double v = (double)values[p] * rf;
-            if (do_cols) v *= pow(sqrt((double)col_counts[indices[p]]), col_pow);
+            if (do_cols) {
+                // a column without nonzeros keeps factor 1 (pow(0, <0) would be inf, and 0 * inf NaN): only stored zeros
+                // meet it, and the reference has dropped them
+                const int32_t cnt = col_counts[indices[p]];
+                if (cnt > 0) v *= pow(sqrt((double)cnt), col_pow);
+            }
             values[p] = (float)v;
         }
     }
@@ -205,12 +213,15 @@ extern "C" int pb200_rescale(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, int
     int blocks = 8 * ctx->num_sms;
     if (do_cols) {
         PB_CUDA(ctx, cudaMemsetAsync(counts, 0, sizeof(int32_t) * (size_t)n_cols, ctx->stream));
-        count_cols_kernel<<<blocks, 256, 0, ctx->stream>>>(indices, nnz, counts);
+        count_cols_kernel<<<blocks, 256, 0, ctx->stream>>>(indices, values, nnz, counts);
         ctx->stats[0] += 1;
         PB_TRY(pb_reduce(ctx, counts, n_cols, PB200_I32));       // row-sharded matrix: column counts are global
     }
-    // NOTE the reference scales rows first and recounts nothing in between: both counts are
-    // structural nnz counts of the same pattern (matrices.py:79, binary=True), so one pass suffices.
+    // NOTE the reference scales rows first, then columns, each pass a sparse product with a diagonal matrix
+    // (models.py:891-895, matrices.py:71-93, binary=True).  The row counts are structural: they include the stored zeros
+    // of the ingested matrix.  The row pass is a sparse product even at row_scaling == 1, and a sparse product stores only
+    // nonzero results, so the column counts see the matrix without its zeros: count_cols_kernel counts values != 0.
+    // Scaling never turns a nonzero into a zero here, so both factors can be applied in one pass; zeros stay stored as 0.
     rescale_kernel<<<blocks, 256, 0, ctx->stream>>>(indptr, indices, values, n_rows, counts,
                                                     row_scaling - 1.0, col_scaling - 1.0, do_rows, do_cols);
     ctx->stats[0] += 1;

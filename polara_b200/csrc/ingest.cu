@@ -87,7 +87,8 @@ __global__ void coo_heads_kernel(const unsigned long long* __restrict__ keys, in
     if (blockIdx.x == 0 && threadIdx.x == 0) head[nnz] = 0;
 }
 
-// every head sums its run of duplicates in sorted (= input, the sort is stable) order and writes the unique entry
+// every head sums its run of duplicates in sorted (= input, the sort is stable) order and writes the unique entry; a sum
+// of zero is kept as a stored zero (coo_matrix(...).tocsr() keeps explicit zeros and duplicates that cancel)
 __global__ void coo_compact_kernel(const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ perm,
                                    const int64_t* __restrict__ slot /* exclusive scan of head */, const void* __restrict__ vals,
                                    int dtype, int64_t nnz, int64_t n_cols, int32_t* __restrict__ indices,
@@ -97,8 +98,8 @@ __global__ void coo_compact_kernel(const unsigned long long* __restrict__ keys, 
     for (; i < nnz; i += stride) {
         const unsigned long long k = keys[i];
         if (k == ~0ull || (i > 0 && keys[i - 1] == k)) continue;
-        double s = 0.0;
-        for (int64_t j = i; j < nnz && keys[j] == k; ++j) s += load_val(vals, dtype, perm[j]);
+        double s = load_val(vals, dtype, perm[i]);      // not 0.0 + ...: a lone -0.0 stays -0.0, as scipy stores it
+        for (int64_t j = i + 1; j < nnz && keys[j] == k; ++j) s += load_val(vals, dtype, perm[j]);
         const int64_t o = slot[i];
         indices[o] = (int32_t)(k % (unsigned long long)n_cols);
         values[o] = (float)s;

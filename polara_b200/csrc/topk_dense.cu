@@ -160,13 +160,20 @@ __global__ void minmax_final_kernel(const double* __restrict__ partial, int nblk
 
 // new values are computed from the ORIGINAL seen scores (the reference gathers them all before it writes, and repeated
 // coordinates are idempotent): gather first, write after
+// min(S) - (max(S_seen) - x) - 1 in the dtype of the scores, one rounding per operation as numpy evaluates it.  mn and
+// mx are elements of S, so narrowing them back to float is exact; __fsub_rn keeps the three float32 steps apart.
+__device__ __forceinline__ float downvote_value(double mn, double mx, float x) {
+    return __fsub_rn(__fsub_rn((float)mn, __fsub_rn((float)mx, x)), 1.0f);
+}
+__device__ __forceinline__ double downvote_value(double mn, double mx, double x) { return mn - (mx - x) - 1.0; }
+
 template <typename T>
 __global__ void downvote_gather_kernel(const T* __restrict__ S, int64_t lds, const int64_t* __restrict__ rows,
                                        const int64_t* __restrict__ cols, int64_t nnz, const double* __restrict__ mm,
                                        T* __restrict__ lowered) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nnz; i += stride)
-        lowered[i] = (T)(mm[0] - (mm[1] - (double)S[rows[i] * lds + cols[i]]) - 1.0);
+        lowered[i] = downvote_value(mm[0], mm[1], S[rows[i] * lds + cols[i]]);
 }
 template <typename T>
 __global__ void downvote_scatter_kernel(T* __restrict__ S, int64_t lds, const int64_t* __restrict__ rows,

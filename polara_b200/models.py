@@ -939,15 +939,17 @@ def hybrid_item_projectors(lower, perm, v):
 
 def _rescale_host(matrix, scaling, axis):
     """rescale_matrix (preprocessing/matrices.py:71-93, binary=True) on a float64 CSR: the lines along ``axis`` scaled by
-    ``sqrt(nnz count) ** (scaling - 1)``."""
+    ``sqrt(count) ** (scaling - 1)``, ``count`` the line's stored entries.  The reference's sparse product with
+    ``diags(...)`` stores only nonzero results, even at ``scaling == 1``, so the result holds no explicit zeros: after
+    the row pass the column counts exclude the stored zeros the row counts include (as pb200_rescale counts them)."""
     import scipy.sparse as sps_
-    if scaling == 1:
-        return matrix
     norm = np.sqrt(np.asarray(matrix.getnnz(axis=axis)).ravel().astype(np.float64))
     factor = np.ones_like(norm)
     factor[norm != 0] = np.power(norm[norm != 0], scaling - 1)
     d = sps_.diags(factor)
-    return (matrix @ d).tocsr() if axis == 0 else (d @ matrix).tocsr()
+    out = (matrix @ d).tocsr() if axis == 0 else (d @ matrix).tocsr()
+    out.eliminate_zeros()
+    return out
 
 
 class _HybridSVDDeviceMixin(_SVDDeviceMixin):

@@ -545,12 +545,15 @@ def test_topk_dense_matches_reference_semantics(eng, dtype, m, n, k):
     # (1) plain top-k == row-wise topsort (scores are tie-free)
     ids = eng.topk_dense(s_dev, k).cpu().numpy()
     np.testing.assert_array_equal(ids, po.get_topk_elements(s.astype(np.float64), k))
-    # (2) in-place downvote == the reference formula; then top-k of the lowered block
+    # (2) in-place downvote == the reference formula evaluated in the input dtype, bit for bit; then top-k of the
+    # lowered block (the lists: from the float64 formula, which orders the seen items by their original score)
     ref = s.astype(np.float64).copy()
     po.downvote_seen_items(ref, rows, cols)
+    exact = s.copy()
+    po.downvote_seen_items(exact, rows, cols)
     low = eng.upload(s.copy())
     eng.downvote_dense(low, eng.upload(rows.astype(np.int64)), eng.upload(cols.astype(np.int64)))
-    np.testing.assert_allclose(low.cpu().numpy(), ref, rtol=1e-6 if dtype == np.float32 else 1e-12)
+    np.testing.assert_array_equal(low.cpu().numpy(), exact)
     ids_low = eng.topk_dense(low, k).cpu().numpy()
     ref_ids = po.get_topk_elements(ref, k)
     np.testing.assert_array_equal(ids_low, ref_ids)
