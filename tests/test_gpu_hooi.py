@@ -8,7 +8,11 @@ Tolerances follow from each kernel's summation order (DESIGN.md §4):
     chain of roundings the kernel's order implies (window kernel: 512 per window + one per carried piece; row-owned kernel:
     len / 8 per warp + the 8 warp partials).
   * fp64 accumulation (pb200_ttm_reduce, the Gram matrix of pb200_tall_svd): ``2^-22 * (scale + |ref|)``.
-  * every kernel is deterministic: a second run is bit-identical."""
+  * every kernel is deterministic: a second run is bit-identical.
+
+These bounds catch a lost window piece or warp partial, not a wrong summation order.  The order itself is checked bit for
+bit against the host emulation of tests/hooi_exact.py in tests/test_gpu_hooi_exact.py (the kernels, the products of a
+real build and the CoFFee lists) and tests/test_cpu_hooi_exact.py (the emulation and its fixtures)."""
 import functools
 
 import numpy as np
@@ -17,6 +21,7 @@ import torch
 
 from oracle import polara_oracle as po
 from tests.helpers import check_topk_against_scores, subspace_gap
+from tests.hooi_exact import TTM_EDGES, WIDTH_ROWS
 
 pytestmark = pytest.mark.gpu
 
@@ -115,22 +120,17 @@ def _run_ttm_case(eng, kernel, lengths, ru, rw, seed=0):
     return out
 
 
-# a row profile for the width sweep: short rows, empty rows, rows around the window size, one long row (> LONG_ROW)
-_WIDTH_ROWS = tuple(int(x) for x in np.r_[[0, 0, 7], np.random.default_rng(1).integers(0, 40, 300), [5000], [0] * 40,
-                                          [700, 513, 511, 0]])
-
-
 @pytest.mark.parametrize("ru,rw", [(3, 2), (5, 24), (4, 32), (3, 43), (4, 60), (4, 64), (3, 86), (4, 128), (5, 103),
                                    (32, 32)])
 def test_ttm_widths_match_f64(eng, ttm_kernel, ru, rw):
     """Every template instance of both TTM kernels: ttm_window_kernel<4|8|16> (width <= 128, <= 256, <= 512) and
     ttm_kernel<4|8|16|32>; the widths sit on and just past each boundary (128 / 129, 256 / 258, 512 / 515) and include the
     C4 mode-0 width 240.  Factors are column slices (ldu = ru + 3, ldw = rw + 1)."""
-    out = _run_ttm_case(eng, ttm_kernel, _WIDTH_ROWS, ru, rw)
+    out = _run_ttm_case(eng, ttm_kernel, WIDTH_ROWS, ru, rw)
     if ru * rw > 512:
         # beyond 512 columns every switch value runs the row-owned kernel: the other value must give the same bits
         eng.set_spmm_kernel("ldg" if ttm_kernel == "window" else "window")
-        other = _run_ttm_case(eng, ttm_kernel, _WIDTH_ROWS, ru, rw)
+        other = _run_ttm_case(eng, ttm_kernel, WIDTH_ROWS, ru, rw)
         assert torch.equal(out, other)
 
 
@@ -141,31 +141,6 @@ def test_ttm_rejects_more_than_1024_columns(eng):
     w = eng.upload(np.ones((1, 32), dtype=np.float32))
     with pytest.raises(ValueError):
         eng.ttm(1, seg, z32, z32, eng.upload(np.ones(4, dtype=np.float32)), u, 33, w, 32)
-
-
-def _skewed_rows():
-    """an item-like grouping: a few rows of 2e4..6e4 nnz (each a dropped 512-nnz piece or 1/8 warp partial away from the
-    bound by far more than 10x), a Zipf tail with many empty rows."""
-    rng = np.random.default_rng(7)
-    tail = np.minimum(rng.zipf(1.6, size=3000) - 1, 3000)
-    return [0, 60_000, 0, 35_001, 20_000] + tail.tolist() + [0, 0]
-
-
-TTM_EDGES = {
-    # segment ends on (512, 1024, 2048, 3072), one before (1023, 4607) and one after (1537, 4609) window boundaries
-    "window_bounds": [512, 0, 511, 1, 513, 511, 0, 1024, 0, 0, 1535, 2, 0],
-    # the same around the row-owned kernel's 2048-nnz blocks
-    "block_bounds": [2048, 0, 2047, 2, 2046, 1, 0, 4096, 0],
-    # 4096 nnz is not a long row, 4097 is (split over 8 warps)
-    "long_row_cutoff": [4096, 4097, 0, 4095, 8193, 1],
-    # runs of more than 32 empty rows: the window kernel reloads its row pointers
-    "empty_runs": [0] * 70 + [1] + [0] * 33 + [600] + [0] * 65,
-    # empty rows first, last and between long ones
-    "empty_around_long": [0] * 5 + [20_000] + [0] * 3 + [9000] + [0] * 40 + [5000] + [0] * 7,
-    # nnz = 0 with rows
-    "no_nnz": [0] * 100,
-    "skewed": _skewed_rows(),
-}
 
 
 @pytest.mark.parametrize("case", sorted(TTM_EDGES))
