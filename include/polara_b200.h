@@ -152,6 +152,24 @@ int pb200_coo_to_csr(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, int64_t nnz
                      const void* vals, int val_dtype, int drop_zeros, int require_sorted_rows,
                      int64_t* indptr_out, int32_t* indices_out, float* values_out, int64_t* nnz_out_host);
 
+/* pb200_coo_to_csr (same CSR, same bits), plus what rewriting the values later needs: perm_out int64 [nnz] = the
+ * stable sort's permutation (sorted position -> input position; the identity when the input was strictly increasing)
+ * and run_ptr_out int64 [nnz_out + 1] = where each stored entry's run of summed duplicates starts in sorted order
+ * (run_ptr_out[nnz_out] = the end of the last run).  Sizes the outputs for the nnz input entries. */
+int pb200_coo_to_csr_runs(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, int64_t nnz,
+                          const int64_t* rows, int64_t row_stride, const int64_t* cols, int64_t col_stride,
+                          const void* vals, int val_dtype, int drop_zeros, int require_sorted_rows,
+                          int64_t* indptr_out, int32_t* indices_out, float* values_out, int64_t* nnz_out_host,
+                          int64_t* perm_out, int64_t* run_ptr_out);
+
+/* values_out[o] (float32, n_unique stored entries) = the sum over entry o's run of table[levels[perm[j]]] (table
+ * float32 [n_levels], levels int64 [nnz] per input triplet), in the order and at the precision pb200_coo_to_csr sums
+ * float32 values: the CSR of pb200_coo_to_csr_runs then holds the same bits as a fresh pb200_coo_to_csr of the float32
+ * weights table[levels].  CoFFee's test matrix at another multilinear rank (models.py:1312-1315).  Synchronises the
+ * stream; a level outside [0, n_levels) is PB200_EINVAL. */
+int pb200_csr_values_from_table(pb200_ctx* ctx, int64_t n_unique, const int64_t* run_ptr, const int64_t* perm,
+                                const int64_t* levels, const float* table, int64_t n_levels, float* values_out);
+
 /* x[i] += delta for i < count (device int64): re-bases the row pointers / user ids of a chunk of a larger matrix. */
 int pb200_shift_i64(pb200_ctx* ctx, int64_t* x, int64_t count, int64_t delta);
 
@@ -406,6 +424,13 @@ int pb200_ttm_reduce(pb200_ctx* ctx, int n_seg, int64_t nnz, const int64_t* seg_
 int pb200_coo_group(pb200_ctx* ctx, int64_t nnz, int64_t n_keys, const int32_t* key,
                     const int32_t* a, const int32_t* b, const float* val,
                     int64_t* seg_ptr, int32_t* a_out, int32_t* b_out, float* val_out);
+
+/* out[n x ldo] (float32) = fp32(V R) for V fp64 [n x K] (ldv) and R fp64 [K x r] (ldr), 1 <= K, r <= 1024; columns
+ * r..ldo-1 are zero.  Each element is acc = 0.0, acc = __dadd_rn(acc, __dmul_rn(V[i,k], R[k,j])) for k ascending, then
+ * __double2float_rn(acc).  The factor rotation of CoffeeModel._check_reduced_rank (models.py:949-963:
+ * factor.dot(rotation)) for the item factor of the Tucker-rank sweep. */
+int pb200_rotate_factor(pb200_ctx* ctx, int64_t n, int K, int r, const double* V, int64_t ldv,
+                        const double* R, int64_t ldr, float* out, int64_t ldo);
 
 #ifdef __cplusplus
 }

@@ -42,6 +42,9 @@ _SIGNATURES = {
     "pb200_spmm_csr": ([ptr, C.POINTER(CsrView), ptr, i64, ptr, i64, C.c_int], C.c_int),
     "pb200_coo_to_csr": ([ptr, i64, i64, i64, ptr, i64, ptr, i64, ptr, C.c_int, C.c_int, C.c_int, ptr, ptr, ptr, C.POINTER(i64)],
                          C.c_int),
+    "pb200_coo_to_csr_runs": ([ptr, i64, i64, i64, ptr, i64, ptr, i64, ptr, C.c_int, C.c_int, C.c_int, ptr, ptr, ptr,
+                               C.POINTER(i64), ptr, ptr], C.c_int),
+    "pb200_csr_values_from_table": ([ptr, i64, ptr, ptr, ptr, ptr, i64, ptr], C.c_int),
     "pb200_topk_dense": ([ptr, ptr, C.c_int, i64, i64, i64, ptr, ptr, C.c_int, ptr, ptr], C.c_int),
     "pb200_downvote_dense": ([ptr, ptr, C.c_int, i64, i64, i64, ptr, ptr, i64], C.c_int),
     "pb200_shift_i64": ([ptr, ptr, i64, i64], C.c_int),
@@ -82,6 +85,7 @@ _SIGNATURES = {
     "pb200_ttm_reduce": ([ptr, C.c_int, i64, ptr, ptr, ptr, ptr, ptr, C.c_int, i64, ptr, C.c_int, i64, ptr, i64],
                          C.c_int),
     "pb200_coo_group": ([ptr, i64, i64, ptr, ptr, ptr, ptr, ptr, ptr, ptr, ptr], C.c_int),
+    "pb200_rotate_factor": ([ptr, i64, C.c_int, C.c_int, ptr, i64, ptr, i64, ptr, i64], C.c_int),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -92,19 +92,61 @@ __global__ void coo_heads_kernel(const unsigned long long* __restrict__ keys, in
 __global__ void coo_compact_kernel(const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ perm,
                                    const int64_t* __restrict__ slot /* exclusive scan of head */, const void* __restrict__ vals,
                                    int dtype, int64_t nnz, int64_t n_cols, int32_t* __restrict__ indices,
-                                   float* __restrict__ values, unsigned long long* __restrict__ ukeys) {
+                                   float* __restrict__ values, unsigned long long* __restrict__ ukeys,
+                                   int64_t* __restrict__ run_ptr /* optional: run_ptr[o + 1] = end of entry o's run */) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (; i < nnz; i += stride) {
         const unsigned long long k = keys[i];
         if (k == ~0ull || (i > 0 && keys[i - 1] == k)) continue;
         double s = load_val(vals, dtype, perm[i]);      // not 0.0 + ...: a lone -0.0 stays -0.0, as scipy stores it
-        for (int64_t j = i + 1; j < nnz && keys[j] == k; ++j) s += load_val(vals, dtype, perm[j]);
+        int64_t j = i + 1;
+        for (; j < nnz && keys[j] == k; ++j) s += load_val(vals, dtype, perm[j]);
         const int64_t o = slot[i];
         indices[o] = (int32_t)(k % (unsigned long long)n_cols);
         values[o] = (float)s;
         ukeys[o] = k;
+        if (run_ptr) run_ptr[o + 1] = j;
     }
+}
+
+__global__ void iota_i64_kernel(int64_t* __restrict__ x, int64_t count) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; i < count; i += stride) x[i] = i;
+}
+
+__global__ void widen_u32_kernel(const uint32_t* __restrict__ x, int64_t count, int64_t* __restrict__ y) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; i < count; i += stride) y[i] = (int64_t)x[i];
+}
+
+// values[o] = the sum of table[levels[perm[j]]] over the run j in [run_ptr[o], run_ptr[o+1]): the first term, then the
+// others added in double in run order, rounded once to float -- the order and precision coo_compact_kernel sums float32
+// values in, and on the sorted path (runs of one) the plain copy coo_convert_sorted_kernel makes.  flags[0] |= 1 for a
+// level outside [0, n_levels) (its entry gets NaN).
+__global__ void csr_values_from_table_kernel(const int64_t* __restrict__ run_ptr, const int64_t* __restrict__ perm,
+                                             const int64_t* __restrict__ levels, const float* __restrict__ table,
+                                             int64_t n_levels, int64_t n_unique, float* __restrict__ values,
+                                             int* __restrict__ flags) {
+    int64_t o = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    int f = 0;
+    for (; o < n_unique; o += stride) {
+        const int64_t a = run_ptr[o], b = run_ptr[o + 1];
+        double s = 0.0;
+        bool bad = false;
+        for (int64_t j = a; j < b; ++j) {
+            const int64_t lv = levels[perm[j]];
+            if (lv < 0 || lv >= n_levels) { bad = true; break; }
+            const double t = (double)table[lv];
+            s = (j == a) ? t : s + t;                    // the first term as it is: a lone -0.0 stays -0.0
+        }
+        if (bad) f = 1;
+        values[o] = bad ? __int_as_float(0x7fc00000) : (float)s;
+    }
+    if (f) atomicOr(flags, f);
 }
 
 __global__ void indptr_from_keys_kernel(const unsigned long long* __restrict__ ukeys, int64_t n_unique, int64_t n_rows,
@@ -138,11 +180,12 @@ extern "C" int pb200_shift_i64(pb200_ctx* ctx, int64_t* x, int64_t count, int64_
     return PB200_OK;
 }
 
-extern "C" int pb200_coo_to_csr(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, int64_t nnz,
-                                const int64_t* rows, int64_t row_stride, const int64_t* cols, int64_t col_stride,
-                                const void* vals, int val_dtype, int drop_zeros, int require_sorted_rows,
-                                int64_t* indptr_out, int32_t* indices_out, float* values_out, int64_t* nnz_out_host) {
-    PB_ENTER(ctx);
+// pb200_coo_to_csr, and with perm_out / run_ptr_out (both or neither) pb200_coo_to_csr_runs
+static int coo_to_csr_impl(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, int64_t nnz,
+                           const int64_t* rows, int64_t row_stride, const int64_t* cols, int64_t col_stride,
+                           const void* vals, int val_dtype, int drop_zeros, int require_sorted_rows,
+                           int64_t* indptr_out, int32_t* indices_out, float* values_out, int64_t* nnz_out_host,
+                           int64_t* perm_out, int64_t* run_ptr_out) {
     PB_REQUIRE(ctx, n_rows >= 0 && n_cols > 0 && nnz >= 0, "coo_to_csr: bad shape");
     PB_REQUIRE(ctx, n_cols < (int64_t)2147483647, "coo_to_csr: column count must fit int32");
     PB_REQUIRE(ctx, nnz < (int64_t)4294967295ll, "coo_to_csr: nnz must be < 2^32");
@@ -152,6 +195,7 @@ extern "C" int pb200_coo_to_csr(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, 
     PB_REQUIRE(ctx, (double)n_rows * (double)n_cols < 1.8e19, "coo_to_csr: n_rows * n_cols must fit 64 bits");
     if (nnz == 0) {
         PB_CUDA(ctx, cudaMemsetAsync(indptr_out, 0, sizeof(int64_t) * (size_t)(n_rows + 1), ctx->stream));
+        if (run_ptr_out) PB_CUDA(ctx, cudaMemsetAsync(run_ptr_out, 0, sizeof(int64_t), ctx->stream));
         *nnz_out_host = 0;
         return PB200_OK;
     }
@@ -174,6 +218,11 @@ extern "C" int pb200_coo_to_csr(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, 
         coo_convert_sorted_kernel<<<blocks, 256, 0, ctx->stream>>>(cols, col_stride, vals, val_dtype, nnz, indices_out, values_out);
         indptr_from_rows_kernel<<<(unsigned)ceil_div64(n_rows + 1, 256), 256, 0, ctx->stream>>>(rows, row_stride, nnz, n_rows, indptr_out);
         ctx->stats[0] += 2;
+        if (perm_out) {                               // every entry is its own run
+            iota_i64_kernel<<<blocks, 256, 0, ctx->stream>>>(perm_out, nnz);
+            iota_i64_kernel<<<blocks, 256, 0, ctx->stream>>>(run_ptr_out, nnz + 1);
+            ctx->stats[0] += 2;
+        }
         PB_CUDA(ctx, cudaGetLastError());
         *nnz_out_host = nnz;
         return PB200_OK;
@@ -201,7 +250,12 @@ extern "C" int pb200_coo_to_csr(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, 
     coo_heads_kernel<<<blocks, 256, 0, ctx->stream>>>(keys_sorted, nnz, head);
     PB_CUDA(ctx, cub::DeviceScan::ExclusiveSum(temp, scan_bytes, head, slot, nnz + 1, ctx->stream));
     coo_compact_kernel<<<blocks, 256, 0, ctx->stream>>>(keys_sorted, perm, slot, vals, val_dtype, nnz, n_cols, indices_out,
-                                                        values_out, ukeys);
+                                                        values_out, ukeys, run_ptr_out);
+    if (perm_out) {
+        PB_CUDA(ctx, cudaMemsetAsync(run_ptr_out, 0, sizeof(int64_t), ctx->stream));
+        widen_u32_kernel<<<blocks, 256, 0, ctx->stream>>>(perm, nnz, perm_out);
+        ctx->stats[0] += 1;
+    }
     int64_t n_unique = 0;
     PB_CUDA(ctx, cudaMemcpyAsync(&n_unique, slot + nnz, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
     PB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -209,5 +263,49 @@ extern "C" int pb200_coo_to_csr(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, 
     ctx->stats[0] += 6;
     PB_CUDA(ctx, cudaGetLastError());
     *nnz_out_host = n_unique;
+    return PB200_OK;
+}
+
+extern "C" int pb200_coo_to_csr(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, int64_t nnz,
+                                const int64_t* rows, int64_t row_stride, const int64_t* cols, int64_t col_stride,
+                                const void* vals, int val_dtype, int drop_zeros, int require_sorted_rows,
+                                int64_t* indptr_out, int32_t* indices_out, float* values_out, int64_t* nnz_out_host) {
+    PB_ENTER(ctx);
+    return coo_to_csr_impl(ctx, n_rows, n_cols, nnz, rows, row_stride, cols, col_stride, vals, val_dtype, drop_zeros,
+                           require_sorted_rows, indptr_out, indices_out, values_out, nnz_out_host, nullptr, nullptr);
+}
+
+extern "C" int pb200_coo_to_csr_runs(pb200_ctx* ctx, int64_t n_rows, int64_t n_cols, int64_t nnz,
+                                     const int64_t* rows, int64_t row_stride, const int64_t* cols, int64_t col_stride,
+                                     const void* vals, int val_dtype, int drop_zeros, int require_sorted_rows,
+                                     int64_t* indptr_out, int32_t* indices_out, float* values_out,
+                                     int64_t* nnz_out_host, int64_t* perm_out, int64_t* run_ptr_out) {
+    PB_ENTER(ctx);
+    PB_REQUIRE(ctx, run_ptr_out != nullptr && (perm_out != nullptr || nnz == 0), "coo_to_csr_runs: outputs are required");
+    return coo_to_csr_impl(ctx, n_rows, n_cols, nnz, rows, row_stride, cols, col_stride, vals, val_dtype, drop_zeros,
+                           require_sorted_rows, indptr_out, indices_out, values_out, nnz_out_host, perm_out, run_ptr_out);
+}
+
+extern "C" int pb200_csr_values_from_table(pb200_ctx* ctx, int64_t n_unique, const int64_t* run_ptr, const int64_t* perm,
+                                           const int64_t* levels, const float* table, int64_t n_levels,
+                                           float* values_out) {
+    PB_ENTER(ctx);
+    PB_REQUIRE(ctx, n_unique >= 0 && n_levels >= 1, "csr_values_from_table: bad sizes");
+    PB_REQUIRE(ctx, n_unique == 0 || (run_ptr && perm && levels && table && values_out),
+               "csr_values_from_table: null pointer");
+    if (n_unique == 0) return PB200_OK;
+    Scratch sc(ctx);
+    int* flags = nullptr;
+    PB_TRY(sc.alloc(&flags, 1));
+    PB_CUDA(ctx, cudaMemsetAsync(flags, 0, sizeof(int), ctx->stream));
+    const int blocks = (int)std::min<int64_t>(ceil_div64(n_unique, 256), 8 * (int64_t)ctx->num_sms);
+    csr_values_from_table_kernel<<<blocks, 256, 0, ctx->stream>>>(run_ptr, perm, levels, table, n_levels, n_unique,
+                                                                  values_out, flags);
+    ctx->stats[0] += 1;
+    PB_CUDA(ctx, cudaGetLastError());
+    int h_flags = 0;
+    PB_CUDA(ctx, cudaMemcpyAsync(&h_flags, flags, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    PB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    PB_REQUIRE(ctx, !h_flags, "csr_values_from_table: a level is outside the table");
     return PB200_OK;
 }

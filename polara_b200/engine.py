@@ -311,6 +311,65 @@ class Engine:
         n = int(out_nnz.value)
         return DeviceCSR(indptr, indices[:n], values[:n], (n_rows, n_cols))
 
+    def coo_to_csr_runs(self, rows, cols, vals, shape, drop_zeros=False, require_sorted_rows=False):
+        """``coo_to_csr`` (same CSR, same bits) plus ``(perm, run_ptr)`` (pb200_coo_to_csr_runs): ``perm`` int64 [nnz] maps
+        sorted positions to input triplets, ``run_ptr`` int64 [csr.nnz + 1] bounds each stored entry's run of summed
+        duplicates.  ``csr_values_from_table`` rewrites the values from them.  Returns ``(csr, perm, run_ptr)``."""
+        nnz = int(rows.shape[0])
+        n_rows, n_cols = int(shape[0]), int(shape[1])
+        if rows.dtype != _I64 or cols.dtype != _I64 or not rows.is_cuda or not cols.is_cuda:
+            raise TypeError("coo_to_csr_runs: rows / cols must be int64 CUDA tensors")
+        if vals is not None and vals.dtype not in (_F32, _F64):
+            raise TypeError("coo_to_csr_runs: values must be float32 or float64")
+        if vals is not None and vals.stride(0) != 1:
+            vals = vals.contiguous()
+        indptr = self.empty((n_rows + 1,), torch.int64)
+        indices = self.empty((max(nnz, 1),), torch.int32)
+        values = self.empty((max(nnz, 1),), torch.float32)
+        perm = self.empty((max(nnz, 1),), torch.int64)
+        run_ptr = self.empty((nnz + 1,), torch.int64)
+        out_nnz = C.c_int64(0)
+        st = self.lib.pb200_coo_to_csr_runs(self.h, n_rows, n_cols, nnz, C.c_void_p(rows.data_ptr()),
+                                            rows.stride(0) if nnz else 1, C.c_void_p(cols.data_ptr()),
+                                            cols.stride(0) if nnz else 1,
+                                            C.c_void_p(vals.data_ptr()) if vals is not None else None,
+                                            1 if (vals is not None and vals.dtype == _F64) else 0, int(bool(drop_zeros)),
+                                            int(bool(require_sorted_rows)), _p(indptr), _p(indices), _p(values),
+                                            C.byref(out_nnz), _p(perm), _p(run_ptr))
+        self._check(st, "coo_to_csr_runs")
+        n = int(out_nnz.value)
+        return DeviceCSR(indptr, indices[:n], values[:n], (n_rows, n_cols)), perm[:nnz], run_ptr[:n + 1]
+
+    def csr_values_from_table(self, a: DeviceCSR, perm, run_ptr, levels, table):
+        """In place: ``a.values`` <- the per-entry sums of ``table[levels]`` over the runs of ``coo_to_csr_runs``
+        (pb200_csr_values_from_table), the bits a fresh ``coo_to_csr`` of the float32 weights ``table[levels]`` gives.
+        ``levels`` int64 CUDA tensor [nnz input triplets], ``table`` float32 CUDA tensor [n_levels]."""
+        if levels.dim() != 1 or levels.shape[0] != perm.shape[0]:
+            raise ValueError("csr_values_from_table: one level per input triplet expected")
+        if table.dim() != 1 or table.shape[0] < 1:
+            raise ValueError("csr_values_from_table: the table must be a non-empty vector")
+        if run_ptr.shape[0] != a.nnz + 1 or a.n_panels != 1:
+            raise ValueError("csr_values_from_table: run bounds do not belong to this CSR")
+        st = self.lib.pb200_csr_values_from_table(self.h, a.nnz, _p(run_ptr, _I64), _p(perm, _I64),
+                                                  _p(levels.contiguous(), _I64), _p(table.contiguous(), _F32),
+                                                  table.shape[0], _p(a.values, _F32))
+        self._check(st, "csr_values_from_table")
+        return a
+
+    def rotate_factor(self, v, rot, out=None):
+        """fp32(V R) zero padded to ``round_up(r, 32)`` columns (pb200_rotate_factor): ``v`` float64 CUDA tensor [n x K]
+        (row stride >= K), ``rot`` float64 CUDA tensor [K x r], K, r <= 1024.  Returns the float32 [n x ld] tensor."""
+        if v.dim() != 2 or rot.dim() != 2 or rot.shape[0] != v.shape[1]:
+            raise ValueError("rotate_factor: expected V [n x K] and R [K x r]")
+        n, k = v.shape
+        r = rot.shape[1]
+        if out is None:
+            out = self.empty((n, round_up(r, 32)))
+        st = self.lib.pb200_rotate_factor(self.h, n, k, r, _p(v, _F64), v.stride(0), _p(rot, _F64), rot.stride(0),
+                                          _p(out, _F32), out.stride(0))
+        self._check(st, "rotate_factor")
+        return out
+
     def shift_i64(self, t, delta):
         """t += delta in place (int64 CUDA tensor): re-basing row pointers / user ids of a chunk."""
         st = self.lib.pb200_shift_i64(self.h, _p(t, _I64), t.numel(), int(delta))

@@ -1317,6 +1317,100 @@ class _CoffeeDeviceMixin(_DeviceModelMixin):
             ids = self._score(p_dev, seen_dev, self._device_factor(f.itemid), self.factors[f.itemid].shape[1])
         return ids.cpu().numpy()
 
+    def tucker_rank_sweep(self, mlranks):
+        """``get_recommendations`` at every multilinear rank ``(r1, r2, r3)`` of ``mlranks`` on the current factors
+        rounded to that rank (``mlrank = t``, models.py:949-980), made from one test-data ingest.  Returns
+        ``{(r1, r2, r3): int64 [n_test_users x topk]}``, honouring ``filter_seen``, ``flattener`` and ``score_kernel``.
+
+        Per triple the core is rounded mode by mode on the host as ``_check_reduced_rank`` rounds it; the user factor,
+        which scoring never reads, is not rotated.  The item factor is rotated on the device (pb200_rotate_factor, once
+        per ``(r1, r2)``) only when ``r2`` is below its width; the feedback factor and the per-level weight table are
+        formed on the host with the expressions of ``get_recommendations``, and the test matrix's values are rewritten
+        from that table (pb200_csr_values_from_table).  At full item rank the lists are bit-identical to the per-triple
+        path; below it the rotated factor is the fixed fp64 chain of pb200_rotate_factor where the per-triple path uses
+        numpy's BLAS, so lists can differ at near-ties (DESIGN.md section 4).  With ``profile_phases`` set the phases of
+        every triple are timed into ``last_sweep_timings``."""
+        if getattr(self, "shard", None) is not None:
+            raise NotImplementedError("Tucker-rank sweep on an item-sharded model")
+        f = self.data.fields
+        entities = (f.userid, f.itemid, f.feedback)
+        w_full = self.factors[f.feedback]
+        flatten_weights(w_full, self.flattener)                 # a flattener the device path lacks raises before any work
+        triples = list(dict.fromkeys(tuple(int(r) for r in t) for t in mlranks))
+        widths = [None if self.factors.get(e) is None else self.factors[e].shape[1] for e in entities]
+        for t in triples:
+            if len(t) != 3 or min(t) < 1 or any(w is not None and r > w for r, w in zip(t, widths)):
+                raise ValueError("sweep ranks must be triples within %s, the widths of the current factors (a larger "
+                                 "rank needs a rebuild); got %s" % (tuple(widths), t))
+        (user, item, fdbk_idx), shape, _ = self._checked_test_input(self._get_test_data)
+        eng = self.engine
+        prof = getattr(self, "profile_phases", False)
+        u_d, i_d = eng.upload(_as_index_array(user)), eng.upload(_as_index_array(item))
+        levels = eng.upload(np.asarray(fdbk_idx, dtype=np.int64))
+        p_dev, perm, run_ptr = eng.coo_to_csr_runs(u_d, i_d, None, shape[:2])
+        seen_dev = (p_dev.indptr, p_dev.indices)              # values never drop entries here: one pattern for all
+        v64, rotated, out, timings = None, {}, {}, []
+        with eng.score_kernel_scope(self.score_kernel):
+            for t in triples:
+                clock = _PhaseClock(prof)
+                core, rot = self.factors["core"], [None, None, None]
+                for mode in range(3):
+                    if widths[mode] is not None and widths[mode] > t[mode]:
+                        rot[mode], core = round_tucker_core(core, mode, t[mode])
+                w = w_full if rot[2] is None else w_full.dot(rot[2])
+                table = (np.asarray(w) @ flatten_weights(w, self.flattener)).astype(np.float32)
+                clock.mark("round_ms", host=True)
+                v_dev = rotated.get(t[:2])
+                if v_dev is None:
+                    if rot[1] is None:
+                        v_dev = self._device_factor(f.itemid)
+                    else:
+                        if v64 is None:
+                            v64 = eng.upload(np.asarray(self.factors[f.itemid], dtype=np.float64))
+                        v_dev = eng.rotate_factor(v64, eng.upload(rot[1]))
+                    rotated[t[:2]] = v_dev
+                clock.mark("rotate_ms")
+                eng.csr_values_from_table(p_dev, perm, run_ptr, levels, eng.upload(table))
+                clock.mark("rewrite_ms")
+                e = eng.spmm(p_dev, v_dev, ell=round_up(t[1], 32))
+                clock.mark("spmm_ms")
+                ids = eng.score_topk(e, v_dev, t[1], self.topk, seen=seen_dev if self.filter_seen else None)
+                clock.mark("score_ms")
+                out[t] = ids.cpu().numpy()
+                timings.append(clock.result(t))
+        if prof:
+            self.last_sweep_timings = timings
+        return out
+
+
+class _PhaseClock:
+    """CUDA events (host clock for ``host=True``) between the phases of one sweep step; inert unless ``on``."""
+
+    def __init__(self, on):
+        self.on, self.marks = on, []
+        if on:
+            self.t_host = time.perf_counter()
+            self.last = torch.cuda.Event(enable_timing=True)
+            self.last.record()
+
+    def mark(self, name, host=False):
+        if not self.on:
+            return
+        ev = torch.cuda.Event(enable_timing=True)
+        ev.record()
+        if host:
+            now = time.perf_counter()
+            self.marks.append((name, (now - self.t_host) * 1e3))
+        else:
+            self.marks.append((name, (self.last, ev)))
+        self.last = ev
+
+    def result(self, key):
+        if not self.on:
+            return None
+        torch.cuda.synchronize()
+        return dict(mlrank=key, **{n: (v if isinstance(v, float) else v[0].elapsed_time(v[1])) for n, v in self.marks})
+
 
 class B200CoffeeModel(_CoffeeDeviceMixin, host.RecommenderModel):
     def __init__(self, *args, **kwargs):

@@ -7,6 +7,12 @@ The reference recomputes the recommendations at every rank; here they come from 
 ingest, the SpMM at the largest rank and, on the sampled protocol, the draw of the unseen items between all ranks.  The
 evaluator then sees the model at each rank with ``_recommendations`` set to that rank's lists.  Item cold-start models
 (users as the target) have a feature transform per rank and take the reference's per-rank loop instead.
+
+:func:`find_optimal_tucker_ranks` does the same for a CoFFee model (pipelines.py:119-160): build once at the largest rank
+of each mode, then evaluate every multilinear rank ``(r1, r2, r3)`` of the grid.  The lists of all triples come from one
+``tucker_rank_sweep`` made before the loop, which ingests the test data once and rotates only the item factor on the
+device.  The evaluator sees ``_mlrank`` set to each triple and ``_recommendations`` set to that triple's lists; unlike
+the reference, ``factors`` stay those of the full build, because rounding the user factor is the cost the sweep removes.
 """
 from __future__ import annotations
 
@@ -14,7 +20,8 @@ from collections.abc import Iterable, Mapping
 
 from .models import sampled_protocol_inputs
 
-__all__ = ["evaluate_models", "find_optimal_svd_rank", "rank_sweep_lists", "set_config"]
+__all__ = ["evaluate_models", "find_optimal_svd_rank", "find_optimal_tucker_ranks", "rank_sweep_lists",
+           "set_config"]
 
 
 def set_config(model, config, convert_nan=True):
@@ -114,3 +121,56 @@ def find_optimal_svd_rank(model, ranks, target_metric, return_scores=False, prot
         scores.name = model.method
         return best_rank, scores.loc[list(ranks)]
     return best_rank
+
+
+def _tucker_grid(tucker_ranks, same_space=False):
+    """The triples pipelines.py:141-148 visits, in its order: ``r1`` of ``tucker_ranks[0]``, ``r2`` of
+    ``tucker_ranks[1]`` (only ``r2 == r1`` with ``same_space``), ``r3`` of ``tucker_ranks[2]``, skipping a triple where
+    one rank exceeds the product of the other two."""
+    return [(r1, r2, r3) for r1 in tucker_ranks[0] for r2 in tucker_ranks[1] if not (same_space and r2 != r1)
+            for r3 in tucker_ranks[2] if not (r1 * r2 < r3 or r1 * r3 < r2 or r2 * r3 < r1)]
+
+
+def find_optimal_tucker_ranks(model, tucker_ranks, target_metric, return_scores=False, config=None, verbose=False,
+                              same_space=False, evaluator=None, iterator=lambda x: x, **kwargs):
+    """pipelines.py:119-160 with the lists of all triples from one ``tucker_rank_sweep`` (see the module docstring).
+    ``model.mlrank`` is set to the largest rank of each mode and the model is built if it is not ready; then
+    ``evaluator(model, target_metric, **kwargs)[model.method]`` (default :func:`evaluate_models`) scores each triple of
+    the grid, ``iterator`` wrapping the ranks of the first mode as in the reference.  During each call the model
+    shows ``_mlrank`` equal to the triple and that triple's lists, but the factors of the full build, not the rounded
+    ones.  ``_mlrank`` and ``factors`` are restored afterwards, also when the evaluator raises; ``verbose`` is restored
+    after the loop.  Returns the best triple and, with ``return_scores``, the Series of scores indexed by
+    ``(r1, r2, r3)``."""
+    import pandas as pd
+    evaluator = evaluator or evaluate_models
+    model_verbose = model.verbose
+    if config:
+        set_config(model, config)
+    model.mlrank = tuple([max(mode_ranks) for mode_ranks in tucker_ranks])
+    if not model._is_ready:
+        model.verbose = verbose
+        model.build()
+    factors = dict(**model.factors)
+    tucker_rank = model.mlrank
+    grid = _tucker_grid(tucker_ranks, same_space)
+    res_score = {}
+    try:
+        lists = model.tucker_rank_sweep(grid) if grid else {}
+        for r1 in iterator(tucker_ranks[0]):
+            for mlrank in _tucker_grid(([r1],) + tuple(tucker_ranks[1:]), same_space):
+                model._mlrank = mlrank
+                model._recommendations = lists[mlrank]
+                res_score[mlrank] = evaluator(model, target_metric, **kwargs)[model.method]
+                model._recommendations = None          # the next triple must not see this triple's lists
+    finally:
+        model._mlrank = tucker_rank
+        model.factors = dict(**factors)
+        model._recommendations = None
+    model.verbose = model_verbose
+    scores = pd.Series(res_score).sort_index()
+    best_mlrank = scores.idxmax()
+    if return_scores:
+        scores.index.names = ["r1", "r2", "r3"]
+        scores.name = model.method
+        return best_mlrank, scores
+    return best_mlrank
