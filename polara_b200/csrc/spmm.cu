@@ -218,6 +218,23 @@ __device__ __forceinline__ int64_t lower_bound_ptr(const int64_t* __restrict__ a
     return lo;
 }
 
+// the same result from a whole warp: each step 32 lanes probe 32 evenly spaced pointers, so 1M rows take 4 dependent
+// loads instead of 20
+__device__ __forceinline__ int64_t lower_bound_ptr_warp(const int64_t* __restrict__ a, int64_t n, int64_t key, int lane) {
+    int64_t lo = 0, hi = n + 1;                          // answer in [lo, hi]; a[hi] >= key or hi == n + 1
+    while (hi - lo > 32) {
+        const int64_t s = (hi - lo + 31) >> 5;
+        const int64_t q = min(lo + (lane + 1) * s, hi) - 1;
+        const uint32_t ge = __ballot_sync(0xffffffffu, __ldg(a + q) >= key);
+        if (ge == 0) return hi;
+        const int f = __ffs(ge) - 1;
+        hi = min(lo + (f + 1) * s, hi) - 1;
+        lo = lo + f * s;
+    }
+    const uint32_t ge = __ballot_sync(0xffffffffu, lo + lane < hi && __ldg(a + lo + lane) >= key);
+    return ge ? lo + __ffs(ge) - 1 : hi;
+}
+
 // LPT  = 32-column groups per row segment (1..4); warp j of the consumers owns columns [32j, 32j+32).
 // NG   = ring depth in groups of 32 staged rows (staged variants).
 // PROD = 0: X rows staged in shared memory by cp.async.bulk (UBLKCP), one bulk copy per row, complete_tx on an mbarrier;
@@ -544,7 +561,7 @@ spmm_window4_kernel(int64_t n_rows, const int64_t* __restrict__ indptr, const in
     int64_t cur;
     bool piece_is_carry;
     {
-        const int64_t lb = b == 0 ? 0 : lower_bound_ptr(indptr, n_rows, w0);
+        const int64_t lb = b == 0 ? 0 : lower_bound_ptr_warp(indptr, n_rows, w0, lane);
         if (lb <= n_rows && (b == 0 || __ldg(indptr + lb) == w0)) { cur = lb; piece_is_carry = false; }
         else { cur = lb - 1; piece_is_carry = true; }
     }
@@ -625,14 +642,32 @@ spmm_window4_kernel(int64_t n_rows, const int64_t* __restrict__ indptr, const in
                 acc.x = fmaf(v2, x2.x, acc.x); acc.y = fmaf(v2, x2.y, acc.y); acc.z = fmaf(v2, x2.z, acc.z); acc.w = fmaf(v2, x2.w, acc.w);
                 acc.x = fmaf(v3, x3.x, acc.x); acc.y = fmaf(v3, x3.y, acc.y); acc.z = fmaf(v3, x3.z, acc.z); acc.w = fmaf(v3, x3.w, acc.w);
             }
-            for (; t < seg_end; t += STEP) {
-                const int i0 = t + hw;
-                const bool ok = i0 < seg_end;                          // an odd tail: the second half-warp sits this one out
-                const int32_t c0 = __shfl_sync(0xffffffffu, c, ok ? i0 : t);
-                float v0 = __shfl_sync(0xffffffffu, v, ok ? i0 : t);
-                if (!ok) v0 = 0.f;
-                const float4 x0 = ok ? gather(c0) : make_float4(0.f, 0.f, 0.f, 0.f);
-                acc.x = fmaf(v0, x0.x, acc.x); acc.y = fmaf(v0, x0.y, acc.y); acc.z = fmaf(v0, x0.z, acc.z); acc.w = fmaf(v0, x0.w, acc.w);
+            if (t < seg_end) {
+                // the segment's tail, at most NT gathers per lane: all are issued before the first is consumed, so a
+                // tail costs one round trip instead of one per gather.  The gathers are unconditional (a predicated
+                // vector load is completed by predicated moves that wait for it): a lane without an nnz of its own
+                // repeats the row of the tail's first nnz, which this instruction reads anyway.
+                constexpr int NT = 4 - STEP % 2;                      // most gathers of a tail: 3 nnz or 4 pairs
+                const int n_tail = (seg_end - t + STEP - 1) / STEP;
+                float4 xt[NT];
+                float vt[NT];
+                bool okt[NT];
+#pragma unroll
+                for (int j = 0; j < NT; ++j) {
+                    const int i0 = t + j * STEP + hw;
+                    okt[j] = i0 < seg_end;                             // an odd tail: the second half-warp sits this one out
+                    const int src = okt[j] ? i0 : t;
+                    vt[j] = __shfl_sync(0xffffffffu, v, src);
+                    xt[j] = gather(__shfl_sync(0xffffffffu, c, src));
+                }
+#pragma unroll
+                for (int j = 0; j < NT; ++j) {
+                    if (j < n_tail) {
+                        const float v0 = okt[j] ? vt[j] : 0.f;
+                        const float4 x0 = okt[j] ? xt[j] : make_float4(0.f, 0.f, 0.f, 0.f);
+                        acc.x = fmaf(v0, x0.x, acc.x); acc.y = fmaf(v0, x0.y, acc.y); acc.z = fmaf(v0, x0.z, acc.z); acc.w = fmaf(v0, x0.w, acc.w);
+                    }
+                }
             }
             t = seg_end;
             touched = true;
